@@ -59,8 +59,10 @@ class GaussianParams(nn.Module):
         shs = t(scene["shs"])
         op = t(scene["opacities"]).clamp(1e-6, 1 - 1e-6)
         self._xyz = nn.Parameter(t(scene["means3D"]).contiguous())
-        self._features_dc = nn.Parameter(shs[:, :1, :].contiguous())
-        self._features_rest = nn.Parameter(shs[:, 1:, :].contiguous())
+        # own storage, not views of shs: with one Gaussian shs[:, 1:, :] is already contiguous, so .contiguous() would
+        # return a view 12 bytes into shs, and the kernels need 16-byte aligned SH blocks
+        self._features_dc = nn.Parameter(shs[:, :1, :].clone(memory_format=torch.contiguous_format))
+        self._features_rest = nn.Parameter(shs[:, 1:, :].clone(memory_format=torch.contiguous_format))
         self._scaling = nn.Parameter(torch.log(t(scene["scales"])).contiguous())
         self._rotation = nn.Parameter(t(scene["rotations"]).contiguous())
         self._opacity = nn.Parameter(torch.log(op / (1 - op)).contiguous())

@@ -26,13 +26,17 @@ def cam_dev(cam):
                 cp=to_dev(cam["campos"], torch.float32))
 
 
+def nan(*shape):
+    return torch.full(shape, float("nan"), device=DEV)
+
+
 def preprocess_forward(sc, cam, scale_modifier=1.0):
+    """Outputs start as NaN / -7 / 0xAB: the kernel promises to write every one of them for every splat."""
     P = sc["means3D"].shape[0]
     d = {k: to_dev(v, torch.float32) for k, v in sc.items()}
     c = cam_dev(cam)
-    out = dict(means2D=torch.empty((P, 2), device=DEV), depths=torch.empty((P,), device=DEV),
-               radii=torch.empty((P,), dtype=torch.int32, device=DEV), conic_opacity=torch.empty((P, 4), device=DEV),
-               rgb=torch.empty((P, 3), device=DEV), clamped=torch.empty((P,), dtype=torch.uint8, device=DEV))
+    out = dict(means2D=nan(P, 2), depths=nan(P), radii=torch.full((P,), -7, dtype=torch.int32, device=DEV),
+               conic_opacity=nan(P, 4), rgb=nan(P, 3), clamped=torch.full((P,), 0xAB, dtype=torch.uint8, device=DEV))
     _lib.call("gs_preprocess_forward", P, cam["sh_degree"], d["means3D"].data_ptr(), d["scales"].data_ptr(),
               float(scale_modifier), d["rotations"].data_ptr(), d["opacities"].data_ptr(), d["shs"].data_ptr(),
               c["V"].data_ptr(), c["PM"].data_ptr(), c["cp"].data_ptr(), cam["image_width"], cam["image_height"],
@@ -45,15 +49,49 @@ def preprocess_forward(sc, cam, scale_modifier=1.0):
 
 def preprocess_backward(d, c, cam, pre, g_means2D, g_conic, g_rgb, scale_modifier=1.0):
     P = d["means3D"].shape[0]
-    out = dict(means3D=torch.empty((P, 3), device=DEV), scales=torch.empty((P, 3), device=DEV),
-               rotations=torch.empty((P, 4), device=DEV), opacities=torch.empty((P, 1), device=DEV),
-               shs=torch.empty((P, 16, 3), device=DEV))
+    out = dict(means3D=nan(P, 3), scales=nan(P, 3), rotations=nan(P, 4), opacities=nan(P, 1), shs=nan(P, 16, 3))
     _lib.call("gs_preprocess_backward", P, cam["sh_degree"], d["means3D"].data_ptr(), d["scales"].data_ptr(),
               float(scale_modifier), d["rotations"].data_ptr(), d["shs"].data_ptr(), c["V"].data_ptr(),
               c["PM"].data_ptr(), c["cp"].data_ptr(), cam["image_width"], cam["image_height"], float(cam["tanfovx"]),
               float(cam["tanfovy"]), pre["radii"].data_ptr(), pre["clamped"].data_ptr(), g_means2D.data_ptr(),
               g_conic.data_ptr(), g_rgb.data_ptr(), out["means3D"].data_ptr(), out["scales"].data_ptr(),
               out["rotations"].data_ptr(), out["opacities"].data_ptr(), out["shs"].data_ptr(), stream())
+    torch.cuda.synchronize()
+    return out
+
+
+def raw_parameters(sc):
+    """The six raw GaussianModel parameters of an activated scene (pipeline.GaussianParams) as plain device tensors."""
+    from gs_b200 import pipeline
+    p = pipeline.GaussianParams(sc, DEV)
+    return [t.detach() for t in p.raw_parameters()]
+
+
+def preprocess_forward_raw(raw, cam, scale_modifier=1.0):
+    """gs_preprocess_forward_raw on raw = raw_parameters(...); outputs pre-filled like preprocess_forward's."""
+    P = raw[0].shape[0]
+    c = cam_dev(cam)
+    out = dict(means2D=nan(P, 2), depths=nan(P), radii=torch.full((P,), -7, dtype=torch.int32, device=DEV),
+               conic_opacity=nan(P, 4), rgb=nan(P, 3), clamped=torch.full((P,), 0xAB, dtype=torch.uint8, device=DEV))
+    _lib.call("gs_preprocess_forward_raw", P, cam["sh_degree"], *(t.data_ptr() for t in raw[:4]), float(scale_modifier),
+              raw[4].data_ptr(), raw[5].data_ptr(), c["V"].data_ptr(), c["PM"].data_ptr(), c["cp"].data_ptr(),
+              cam["image_width"], cam["image_height"], float(cam["tanfovx"]), float(cam["tanfovy"]),
+              out["means2D"].data_ptr(), out["depths"].data_ptr(), out["radii"].data_ptr(),
+              out["conic_opacity"].data_ptr(), out["rgb"].data_ptr(), out["clamped"].data_ptr(), stream())
+    torch.cuda.synchronize()
+    return out
+
+
+def preprocess_backward_raw(raw, cam, pre, g_means2D, g_conic, g_rgb, scale_modifier=1.0):
+    """gs_preprocess_backward_raw -> [d_xyz, d_features_dc, d_features_rest, d_scaling, d_rotation, d_opacity]."""
+    P = raw[0].shape[0]
+    c = cam_dev(cam)
+    out = [torch.full_like(t, float("nan")) for t in raw]
+    _lib.call("gs_preprocess_backward_raw", P, cam["sh_degree"], *(t.data_ptr() for t in raw[:4]), float(scale_modifier),
+              raw[4].data_ptr(), raw[5].data_ptr(), c["V"].data_ptr(), c["PM"].data_ptr(), c["cp"].data_ptr(),
+              cam["image_width"], cam["image_height"], float(cam["tanfovx"]), float(cam["tanfovy"]),
+              pre["radii"].data_ptr(), pre["clamped"].data_ptr(), g_means2D.data_ptr(), g_conic.data_ptr(),
+              g_rgb.data_ptr(), *(t.data_ptr() for t in out), stream())
     torch.cuda.synchronize()
     return out
 

@@ -414,3 +414,14 @@ def test_quantised_buffer_sizes():
     assert len(xs) <= 8          # a 20 % range of instance counts -> a handful of sizes
     for a, b in zip(xs, xs[1:]):
         assert b > a
+
+
+@pytest.mark.parametrize("n", [1, 2, 5])
+def test_gaussian_params_sh_blocks_own_aligned_storage(n):
+    """The _raw / _batched kernels need 16-byte aligned SH blocks.  With one Gaussian shs[:, 1:, :] is already
+    contiguous, so .contiguous() would hand back a view 12 bytes into the SH tensor."""
+    from gs_b200 import pipeline, synthetic as syn
+    p = pipeline.GaussianParams(syn.make_scene(n, 64, 48, seed=2), "cpu")
+    for t in (p._features_dc, p._features_rest):
+        assert t.is_contiguous() and t.storage_offset() == 0 and t.data_ptr() % 16 == 0
+    assert p._features_dc.untyped_storage().data_ptr() != p._features_rest.untyped_storage().data_ptr()

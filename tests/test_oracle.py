@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import torch
 
+import proj_cases
 import torch_ref
 from gs_b200 import synthetic as syn
 from oracle.oracle import Oracle
@@ -96,28 +97,56 @@ def test_backward_matches_torch_autograd(o64):
 
 
 def test_guard_band_clamp_is_straight_through(o64):
-    """Gaussians outside the 1.3x guard band still project; their clamped ratio carries no gradient."""
-    cam = syn.make_camera(96, 64)
+    """Gaussians outside the 1.3x guard band still project; their clamped ratio carries no gradient.  Every camera x SH
+    degree 0..3 x scale_modifier {1, 0.6}.  "yaw": the synthetic camera at the origin with splats beyond the band on x.
+    0..5: the posed cameras of cameras.npz (translated, re-centred, fx != fy) with the region mix of proj_cases (interior,
+    guard band on x / y / both and at its edge, both sides of the near plane, behind, off-screen, flat, sub-pixel,
+    negative DC)."""
+    for camera in ["yaw"] + list(range(proj_cases.N_GOLDEN)):
+        for deg in range(4):
+            for mod in (1.0, 0.6):
+                _guard_band_case(o64, camera, deg, mod)
+
+
+def _guard_band_case(o64, camera, deg, mod):
+    case = f"camera {camera}, degree {deg}, scale_modifier {mod}"
     rng = np.random.default_rng(5)
-    n = 64
-    z = rng.uniform(2, 4, n)
-    x = rng.choice([-1.0, 1.0], n) * rng.uniform(1.32, 1.5, n) * z * cam["tanfovx"]
-    sc = dict(means3D=np.stack([x, rng.uniform(-.2, .2, n) * z, z], 1), scales=np.exp(rng.normal(-0.5, 0.3, (n, 3))),
-              rotations=syn.make_scene(n, 96, 64, seed=1)["rotations"].astype(np.float64),
-              opacities=rng.uniform(0.3, 0.9, (n, 1)), shs=rng.normal(0, 0.5, (n, 16, 3)))
-    pre = o64.preprocess_forward(sc["means3D"], sc["scales"], sc["rotations"], sc["shs"], sc["opacities"], cam)
-    assert (pre["radii"] > 0).sum() > 10
+    if camera == "yaw":
+        cam = syn.make_camera(96, 64, sh_degree=deg)
+        n = 64
+        z = rng.uniform(2, 4, n)
+        x = rng.choice([-1.0, 1.0], n) * rng.uniform(1.32, 1.5, n) * z * cam["tanfovx"]
+        sc = dict(means3D=np.stack([x, rng.uniform(-.2, .2, n) * z, z], 1), scales=np.exp(rng.normal(-0.5, 0.3, (n, 3))),
+                  rotations=syn.make_scene(n, 96, 64, seed=1)["rotations"].astype(np.float64),
+                  opacities=rng.uniform(0.3, 0.9, (n, 1)), shs=rng.normal(0, 0.5, (n, 16, 3)))
+    else:
+        cam = proj_cases.golden_camera(camera, 96, 64, sh_degree=deg)
+        n = 400
+        sc, _ = proj_cases.region_scene(cam, n, seed=10 * camera + deg)
+        sc = {k: v.astype(np.float64) for k, v in sc.items()}
+    W, H = cam["image_width"], cam["image_height"]
+    pre = o64.preprocess_forward(sc["means3D"], sc["scales"], sc["rotations"], sc["shs"], sc["opacities"], cam,
+                                 scale_modifier=mod)
+    vis_np = pre["radii"] > 0
+    tx, ty, tz = (np.asarray(c, np.float64) for c in proj_cases.view_coords32(cam, sc["means3D"]))
+    beyond = vis_np & ((np.abs(tx / tz) > 1.3 * cam["tanfovx"]) | (np.abs(ty / tz) > 1.3 * cam["tanfovy"]))
+    assert vis_np.sum() > 10 and beyond.sum() >= 3, case
     gm, gc, gr = rng.normal(size=(n, 2)), rng.normal(size=(n, 4)), rng.normal(size=(n, 3))
     pb = o64.preprocess_backward(sc["means3D"], sc["scales"], sc["rotations"], sc["shs"], sc["opacities"], cam,
-                                 pre["radii"], pre["clamped"], gm, gc, gr)
+                                 pre["radii"], pre["clamped"], gm, gc, gr, scale_modifier=mod)
     tp = {k: torch.tensor(v, requires_grad=True) for k, v in sc.items()}
-    m2, co, col = torch_ref.preprocess(tp["means3D"], tp["scales"], tp["rotations"], tp["shs"], tp["opacities"], cam)
-    vis = torch.tensor(pre["radii"] > 0)
-    ndc_scale = torch.tensor([2.0 / 96, 2.0 / 64])
+    m2, co, col = torch_ref.preprocess(tp["means3D"], tp["scales"], tp["rotations"], tp["shs"], tp["opacities"], cam,
+                                       scale_modifier=mod)
+    vis = torch.tensor(vis_np)
+    ndc_scale = torch.tensor([2.0 / W, 2.0 / H], dtype=torch.float64)
     L = ((m2 * ndc_scale * torch.tensor(gm)).sum(1) + (co * torch.tensor(gc)).sum(1) + (col * torch.tensor(gr)).sum(1))
     L[vis].sum().backward()
     for k in ("means3D", "scales", "rotations", "shs", "opacities"):
-        np.testing.assert_allclose(pb[k], tp[k].grad.numpy(), rtol=2e-6, atol=1e-9 * (1 + np.abs(pb[k]).max()), err_msg=k)
+        g = tp[k].grad.numpy()
+        assert np.abs(g).max() > 0, (k, case)
+        np.testing.assert_allclose(pb[k], g, rtol=1e-9, atol=1e-12 * np.abs(g).max(), err_msg=f"{k}, {case}")
+    nc = (deg + 1) ** 2
+    assert (pb["shs"][:, nc:] == 0).all(), case
 
 
 def test_finite_differences_whole_step(o64):
