@@ -19,8 +19,7 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
           "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 # translation units whose fp32 chain must match the oracle op for op (tile indices bit-exact)
-PER_FILE = {"preprocess.cu": ["-fmad=false"], "preprocess_raw.cu": ["-fmad=false"],
-            "preprocess_batched.cu": ["-fmad=false"]}
+PER_FILE = {"preprocess.cu": ["-fmad=false"]}
 
 
 def nvcc():

@@ -98,6 +98,19 @@ def _timed(collector, key, start, end):
     collector[key] = v.value() if os.environ.get("GS_B200_EAGER_TIMING") == "1" else v
 
 
+def _screen_outputs(lead, dev):
+    """Empty (means2D, depths, radii, conic_opacity, rgb, clamped) of a preprocess forward; lead = (P,) or (B, P)."""
+    f32 = torch.float32
+    return (torch.empty((*lead, 2), dtype=f32, device=dev), torch.empty(lead, dtype=f32, device=dev),
+            torch.empty(lead, dtype=torch.int32, device=dev), torch.empty((*lead, 4), dtype=f32, device=dev),
+            torch.empty((*lead, 3), dtype=f32, device=dev), torch.empty(lead, dtype=torch.uint8, device=dev))
+
+
+def _grad_or_zeros(g, shape, dev):
+    """An incoming gradient as contiguous fp32, or zeros where autograd passes None for an unused output."""
+    return torch.zeros(shape, dtype=torch.float32, device=dev) if g is None else _f32c(g, "grad")
+
+
 class _PreprocessGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, scales, rotations, shs, opacities, rs):
@@ -112,12 +125,7 @@ class _PreprocessGaussians(torch.autograd.Function):
             raise ValueError("inconsistent Gaussian parameter shapes")
         dev = means3D.device
         vm, pm, cp = _f32c(rs.viewmatrix, "viewmatrix"), _f32c(rs.projmatrix, "projmatrix"), _f32c(rs.campos, "campos")
-        means2D = torch.empty((P, 2), dtype=torch.float32, device=dev)
-        depths = torch.empty((P,), dtype=torch.float32, device=dev)
-        radii = torch.empty((P,), dtype=torch.int32, device=dev)
-        conic_opacity = torch.empty((P, 4), dtype=torch.float32, device=dev)
-        rgb = torch.empty((P, 3), dtype=torch.float32, device=dev)
-        clamped = torch.empty((P,), dtype=torch.uint8, device=dev)
+        means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((P,), dev)
         _lib.call("gs_preprocess_forward", P, int(rs.sh_degree), means3D.data_ptr(), scales.data_ptr(),
                   float(rs.scale_modifier), rotations.data_ptr(), opacities.data_ptr(), shs.data_ptr(), vm.data_ptr(),
                   pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
@@ -136,11 +144,8 @@ class _PreprocessGaussians(torch.autograd.Function):
         vm, pm, cp = ctx.cam
         P = means3D.shape[0]
         dev = means3D.device
-
-        def z(g, shape):
-            return torch.zeros(shape, dtype=torch.float32, device=dev) if g is None else _f32c(g, "grad")
-
-        g_means2D, g_rgb, g_conic_opacity = z(g_means2D, (P, 2)), z(g_rgb, (P, 3)), z(g_conic_opacity, (P, 4))
+        g_means2D, g_rgb = _grad_or_zeros(g_means2D, (P, 2), dev), _grad_or_zeros(g_rgb, (P, 3), dev)
+        g_conic_opacity = _grad_or_zeros(g_conic_opacity, (P, 4), dev)
         d_means3D = torch.empty((P, 3), dtype=torch.float32, device=dev)
         d_scales = torch.empty((P, 3), dtype=torch.float32, device=dev)
         d_rot = torch.empty((P, 4), dtype=torch.float32, device=dev)
@@ -176,12 +181,7 @@ class _PreprocessGaussiansRaw(torch.autograd.Function):
             raise ValueError("inconsistent Gaussian parameter shapes")
         dev = xyz.device
         vm, pm, cp = _f32c(rs.viewmatrix, "viewmatrix"), _f32c(rs.projmatrix, "projmatrix"), _f32c(rs.campos, "campos")
-        means2D = torch.empty((P, 2), dtype=torch.float32, device=dev)
-        depths = torch.empty((P,), dtype=torch.float32, device=dev)
-        radii = torch.empty((P,), dtype=torch.int32, device=dev)
-        conic_opacity = torch.empty((P, 4), dtype=torch.float32, device=dev)
-        rgb = torch.empty((P, 3), dtype=torch.float32, device=dev)
-        clamped = torch.empty((P,), dtype=torch.uint8, device=dev)
+        means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((P,), dev)
         _lib.call("gs_preprocess_forward_raw", P, int(rs.sh_degree), xyz.data_ptr(), f_dc.data_ptr(), f_rest.data_ptr(),
                   scaling.data_ptr(), float(rs.scale_modifier), rotation.data_ptr(), opacity.data_ptr(), vm.data_ptr(),
                   pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
@@ -200,11 +200,8 @@ class _PreprocessGaussiansRaw(torch.autograd.Function):
         vm, pm, cp = ctx.cam
         P = xyz.shape[0]
         dev = xyz.device
-
-        def z(g, shape):
-            return torch.zeros(shape, dtype=torch.float32, device=dev) if g is None else _f32c(g, "grad")
-
-        g_means2D, g_rgb, g_conic_opacity = z(g_means2D, (P, 2)), z(g_rgb, (P, 3)), z(g_conic_opacity, (P, 4))
+        g_means2D, g_rgb = _grad_or_zeros(g_means2D, (P, 2), dev), _grad_or_zeros(g_rgb, (P, 3), dev)
+        g_conic_opacity = _grad_or_zeros(g_conic_opacity, (P, 4), dev)
         d = [torch.empty_like(t) for t in (xyz, f_dc, f_rest, scaling, rotation, opacity)]
         _lib.call("gs_preprocess_backward_raw", P, int(rs.sh_degree), xyz.data_ptr(), f_dc.data_ptr(), f_rest.data_ptr(),
                   scaling.data_ptr(), float(rs.scale_modifier), rotation.data_ptr(), opacity.data_ptr(), vm.data_ptr(),
@@ -823,12 +820,7 @@ class _PreprocessBatched(torch.autograd.Function):
             raise ValueError("features must be (P,1,3)/(P,15,3) and cams (B,40)")
         W, H, D, mod = meta
         dev = xyz.device
-        means2D = torch.empty((B, P, 2), dtype=torch.float32, device=dev)
-        depths = torch.empty((B, P), dtype=torch.float32, device=dev)
-        radii = torch.empty((B, P), dtype=torch.int32, device=dev)
-        conic_opacity = torch.empty((B, P, 4), dtype=torch.float32, device=dev)
-        rgb = torch.empty((B, P, 3), dtype=torch.float32, device=dev)
-        clamped = torch.empty((B, P), dtype=torch.uint8, device=dev)
+        means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((B, P), dev)
         _lib.call("gs_preprocess_forward_batched", B, P, int(D), xyz.data_ptr(), f_dc.data_ptr(), f_rest.data_ptr(),
                   scaling.data_ptr(), float(mod), rotation.data_ptr(), opacity.data_ptr(), cams.data_ptr(), int(W),
                   int(H), means2D.data_ptr(), depths.data_ptr(), radii.data_ptr(), conic_opacity.data_ptr(),
@@ -844,11 +836,8 @@ class _PreprocessBatched(torch.autograd.Function):
         W, H, D, mod = ctx.meta
         P, B = xyz.shape[0], cams.shape[0]
         dev = xyz.device
-
-        def z(g, shape):
-            return torch.zeros(shape, dtype=torch.float32, device=dev) if g is None else _f32c(g, "grad")
-
-        g_means2D, g_rgb, g_conic_opacity = z(g_means2D, (B, P, 2)), z(g_rgb, (B, P, 3)), z(g_conic_opacity, (B, P, 4))
+        g_means2D, g_rgb = _grad_or_zeros(g_means2D, (B, P, 2), dev), _grad_or_zeros(g_rgb, (B, P, 3), dev)
+        g_conic_opacity = _grad_or_zeros(g_conic_opacity, (B, P, 4), dev)
         d = [torch.empty_like(t) for t in (xyz, f_dc, f_rest, scaling, rotation, opacity)]
         _lib.call("gs_preprocess_backward_batched", B, P, int(D), xyz.data_ptr(), f_dc.data_ptr(), f_rest.data_ptr(),
                   scaling.data_ptr(), float(mod), rotation.data_ptr(), opacity.data_ptr(), cams.data_ptr(), int(W),

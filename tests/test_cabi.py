@@ -95,6 +95,68 @@ def test_argument_errors_are_reported_not_crashed(lib):
     assert lib.gs_adam_step(0, None, None, None, None, None, None, None, None, None, None, ctypes.c_float(1.0), None) == 0
 
 
+PREPROCESS_ARGS = r"""
+import ctypes, json, sys
+sys.path.insert(0, %(pkg)r)
+from gs_b200 import _lib
+lib = _lib.load()
+FAKE = 1 << 20   # a 16-byte aligned address that is never dereferenced: no device is visible to this process
+# the int arguments of each entry point in order, and the index (among its pointers) of a 16-byte aligned one
+FORMS = {"gs_preprocess_forward": ("P sh W H", 2), "gs_preprocess_backward": ("P sh W H", 2),
+         "gs_preprocess_forward_raw": ("P sh W H", 4), "gs_preprocess_backward_raw": ("P sh W H", 4),
+         "gs_preprocess_forward_batched": ("B P sh W H", 4), "gs_preprocess_backward_batched": ("B P sh W H", 4)}
+
+def call(name, ptr=None, **ints):
+    names, _ = FORMS[name]
+    vals = dict(dict(B=1, P=8, sh=3, W=16, H=16), **ints)
+    ivals = [vals[n] for n in names.split()]
+    args, k = [], 0
+    argtypes = _lib.SIGNATURES[name][1]
+    for j, t in enumerate(argtypes):
+        if t is ctypes.c_int:
+            args.append(ivals.pop(0))
+        elif t is ctypes.c_float:
+            args.append(1.0)
+        elif j == len(argtypes) - 1:
+            args.append(None)                     # stream
+        else:
+            args.append((ptr or {}).get(k, FAKE))
+            k += 1
+    return getattr(lib, name)(*args)
+
+out = {}
+for name, (names, aligned) in FORMS.items():
+    r = out[name] = {"negative P": call(name, P=-1), "sh_degree 4": call(name, sh=4),
+                     "null pointer": call(name, ptr={0: None}), "misaligned": call(name, ptr={aligned: FAKE + 4}),
+                     "P 0, null pointers": call(name, P=0, ptr={k: None for k in range(40)}),
+                     "P 0, no image": call(name, P=0, W=0), "valid": call(name)}
+    if "batched" in name:
+        r["B 0"], r["B 65"] = call(name, B=0), call(name, B=65)
+print(json.dumps(out))
+"""
+
+
+def test_preprocess_argument_checks(lib):
+    """The six preprocess entry points refuse bad sizes, pointers and alignment before any launch.  The calls run in a
+    process that sees no device, so a check that stops working ends in a launch error and never touches one."""
+    import json
+    import subprocess
+    import sys
+    code = PREPROCESS_ARGS % dict(pkg=os.path.join(ROOT, "grendel-gs_b200"))
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300,
+                       env=dict(os.environ, CUDA_VISIBLE_DEVICES=""))
+    assert r.returncode == 0, r.stderr[-3000:]
+    out = json.loads(r.stdout.strip().splitlines()[-1])
+    assert len(out) == 6
+    for name, rc in out.items():
+        for case in ("negative P", "sh_degree 4", "null pointer", "misaligned") + (("B 0", "B 65") * ("batched" in name)):
+            assert rc[case] == -1, (name, case, rc[case])              # GS_EINVAL
+        assert rc["P 0, null pointers"] == 0, name                      # GS_OK: nothing to do
+        assert rc["valid"] == -2, name                                  # GS_ECUDA: passed every check, no device
+        # gs_preprocess_forward has always refused an empty image, even with P == 0; the others accept it
+        assert rc["P 0, no image"] == (-1 if name == "gs_preprocess_forward" else 0), name
+
+
 def test_dropin_package_exports_reference_names():
     import diff_gaussian_rasterization as d
     from simple_knn._C import distCUDA2  # noqa: F401

@@ -1,7 +1,7 @@
 """-m gpu: the projection entry points against the CPU oracle with posed cameras and region-controlled scenes.
 
 gs_preprocess_{forward,backward}, their _raw (fused activation) and _batched forms all run project()
-(csrc/preprocess_common.cuh).  The other parity tests use a camera at the origin that only yaws, fx == fy, splats well
+(csrc/preprocess.cu).  The other parity tests use a camera at the origin that only yaws, fx == fy, splats well
 inside the image and scale_modifier 1.  Here every case uses a posed camera of tests/golden/cameras.npz (translation,
 re-centring, fovx != fovy) and the region mix of proj_cases.region_scene: interior, the guard band on x / y / both and
 within ulps of its edge, both sides of the near plane, behind, off-screen, flat discs, sub-pixel splats and negative DC
