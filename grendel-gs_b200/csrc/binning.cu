@@ -88,7 +88,9 @@ k_count_tiles(int P, int W, int H, const float *__restrict__ means2D, const floa
         const float bb = co.y * co.y, bb_err = __fmaf_rn(co.y, co.y, -bb);
         const float det = __fmaf_rn(co.x, co.z, -bb) - bb_err;
         float ex = -1.f, ey = -1.f;  // never contributes
-        if (t > 0.f) {
+        // t == 0 is a live splat: fl(1/255) is the one opacity whose 255 o rounds to exactly 1 (thr = -0), and it lies
+        // above 1/255, so the pixel on its mean (power = +0) blends it -- as the alpha >= 1/255 test does
+        if (t >= 0.f) {
             if (!no_cull && det > 0.f && co.x > 0.f && co.z > 0.f) {
                 ex = sqrtf(t * co.z / det) * 1.02f + 0.5f;
                 ey = sqrtf(t * co.x / det) * 1.02f + 0.5f;

@@ -96,9 +96,10 @@ def preprocess_backward_raw(raw, cam, pre, g_means2D, g_conic, g_rgb, scale_modi
     return out
 
 
-def render_forward(H, W, means2D, conic_opacity, rgb, depths, radii, compute_locally, bg, seg=True):
+def render_forward(H, W, means2D, conic_opacity, rgb, depths, radii, compute_locally, bg, seg=True, stats=True):
     """All tensors on the device. Returns a dict holding every intermediate of the binning + blend.
-    seg=False: forward-only call (no segment workspace; a backward then runs the tile-parallel kernel)."""
+    seg=False: forward-only call (no segment workspace; a backward then runs the tile-parallel kernel).
+    stats=False: no statistics pointer (the forward's non-statistics instantiation)."""
     P = means2D.shape[0]
     T = ((H + 15) // 16) * ((W + 15) // 16)
     cl = compute_locally.to(torch.uint8).contiguous()
@@ -122,14 +123,14 @@ def render_forward(H, W, means2D, conic_opacity, rgb, depths, radii, compute_loc
     image = torch.full((3, H, W), float("nan"), device=DEV)
     final_T = torch.zeros((H, W), device=DEV)
     n_contrib = torch.zeros((H, W), dtype=torch.int32, device=DEV)
-    stats = torch.zeros((3,), dtype=torch.int64, device=DEV)
+    stats = torch.zeros((3,), dtype=torch.int64, device=DEV) if stats else None
     segb = _lib.query("gs_render_seg_bytes", R, T) if seg else 0
     # NaN-filled: the backward must only read checkpoints the forward wrote
     seg_ws = torch.full((segb // 4,), float("nan"), device=DEV).view(torch.uint8) if seg else None
     _lib.call("gs_render_forward", P, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(), order.data_ptr(),
               offsets.data_ptr(), rec.data_ptr(), bg_t.data_ptr(), tiles[0].data_ptr(), ids[0].data_ptr(),
               tiles[1].data_ptr(), ids[1].data_ptr(), sort_temp.data_ptr(), sb, ranges.data_ptr(), image.data_ptr(),
-              final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(seg_ws), segb, stream())
+              final_T.data_ptr(), n_contrib.data_ptr(), _lib.ptr(stats), _lib.ptr(seg_ws), segb, stream())
     torch.cuda.synchronize()
     # the 64-bit keys of the published algorithm, rebuilt from the sorted (tile, splat id) pairs
     ids_s, tiles_s = ids[1][:R].to(torch.int64) & 0xffffffff, tiles[1][:R].to(torch.int64) & 0xffffffff
@@ -148,6 +149,59 @@ def render_backward(f, dL_dimage):
               f["cl"].data_ptr(), f["ranges"].data_ptr(), f["ids_buf"].data_ptr(), f["final_T"].data_ptr(),
               f["n_contrib"].data_ptr(), dL_dimage.data_ptr(), _lib.ptr(f["seg_ws"]), f["seg_bytes"], out["means2D"].data_ptr(),
               out["conic_opacity"].data_ptr(), out["rgb"].data_ptr(), stream())
+    torch.cuda.synchronize()
+    return out
+
+
+def render_forward_batched(H, W, views, bg):
+    """gs_render_count_batched + gs_render_forward_batched over views = [(means2D, conic_opacity, rgb, depths, radii,
+    compute_locally)] (device tensors; a view may hold no splat).  Outputs start filled like render_forward's."""
+    B = len(views)
+    T = ((H + 15) // 16) * ((W + 15) // 16)
+    cat = [torch.cat([v[q] for v in views]).contiguous() for q in range(5)]
+    cl = torch.cat([v[5].to(torch.uint8).reshape(-1) for v in views]).contiguous()
+    counts = [int(v[0].shape[0]) for v in views]
+    vs = (C.c_int32 * (B + 1))(*np.concatenate([[0], np.cumsum(counts)]).astype(int).tolist())
+    P = int(sum(counts))
+    bg_t = to_dev(np.asarray(bg, np.float32))
+    offsets = torch.empty((max(P, 1),), dtype=torch.int32, device=DEV)
+    order = torch.empty((max(P, 1),), dtype=torch.int32, device=DEV)
+    rec = torch.empty((max(P, 1), 12), dtype=torch.float32, device=DEV)
+    tb = _lib.query("gs_render_count_temp_bytes", P)
+    temp = torch.empty((tb,), dtype=torch.uint8, device=DEV)
+    R = C.c_int64(0)
+    _lib.call("gs_render_count_batched", B, vs, H, W, *(t.data_ptr() for t in cat[:4]), cat[4].data_ptr(), cl.data_ptr(),
+              order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), temp.data_ptr(), tb, C.byref(R), stream())
+    R = int(R.value)
+    Ra = max(R, 1)
+    tiles = torch.zeros((2, Ra), dtype=torch.int32, device=DEV)
+    ids = torch.zeros((2, Ra), dtype=torch.int32, device=DEV)
+    sb = _lib.query("gs_render_sort_temp_bytes", R)
+    sort_temp = torch.empty((sb,), dtype=torch.uint8, device=DEV)
+    ranges = torch.empty((B * T, 2), dtype=torch.int32, device=DEV)
+    image = torch.full((B, 3, H, W), float("nan"), device=DEV)
+    final_T = torch.zeros((B, H, W), device=DEV)
+    n_contrib = torch.zeros((B, H, W), dtype=torch.int32, device=DEV)
+    stats = torch.zeros((B, 3), dtype=torch.int64, device=DEV)
+    segb = _lib.query("gs_render_seg_bytes", R, B * T)
+    seg_ws = torch.full((segb // 4,), float("nan"), device=DEV).view(torch.uint8)
+    _lib.call("gs_render_forward_batched", B, vs, R, H, W, cat[0].data_ptr(), cat[4].data_ptr(), cl.data_ptr(),
+              order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg_t.data_ptr(), tiles[0].data_ptr(), ids[0].data_ptr(),
+              tiles[1].data_ptr(), ids[1].data_ptr(), sort_temp.data_ptr(), sb, ranges.data_ptr(), image.data_ptr(),
+              final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), seg_ws.data_ptr(), segb, stream())
+    torch.cuda.synchronize()
+    return dict(B=B, P=P, R=R, H=H, W=W, rec=rec, bg=bg_t, cl=cl, ranges=ranges, ids_buf=ids[1], image=image,
+                final_T=final_T, n_contrib=n_contrib, stats=stats, seg_ws=seg_ws, seg_bytes=segb, counts=counts)
+
+
+def render_backward_batched(f, dL_dimage):
+    P = f["P"]
+    out = dict(means2D=torch.full((P, 2), float("nan"), device=DEV), conic_opacity=torch.full((P, 4), float("nan"), device=DEV),
+               rgb=torch.full((P, 3), float("nan"), device=DEV))
+    _lib.call("gs_render_backward_batched", f["B"], P, f["R"], f["H"], f["W"], f["rec"].data_ptr(), f["bg"].data_ptr(),
+              f["cl"].data_ptr(), f["ranges"].data_ptr(), f["ids_buf"].data_ptr(), f["final_T"].data_ptr(),
+              f["n_contrib"].data_ptr(), dL_dimage.data_ptr(), f["seg_ws"].data_ptr(), f["seg_bytes"],
+              out["means2D"].data_ptr(), out["conic_opacity"].data_ptr(), out["rgb"].data_ptr(), stream())
     torch.cuda.synchronize()
     return out
 
