@@ -12,7 +12,7 @@
 //      split's block of normal draws (plane 4); the plane totals go back to the host once;
 //   3. k_densify_gather: every tensor (6 parameters, 12 moments, send_to_gpui_cnt) is read once and written to its
 //      output rows, with the split's two transforms applied on the fly (position: R(q) (s * z) + x, scale:
-//      log(s / 1.6)).
+//      log(s * fl32(1 / 1.6))).
 // Byte / index work plus a few transcendentals: HBM bound, ~(3 x 236 + 4 W) B read and written per Gaussian.
 #include <cub/cub.cuh>
 
@@ -20,6 +20,10 @@
 
 #define DN_THREADS 256
 #define DN_PLANES 5
+// a split child's scale is get_scaling / (0.8 N) with N = 2.  On CUDA, torch divides a tensor by a Python scalar by
+// multiplying with the scalar's fp32 reciprocal, fl32(1 / 1.6f) = 0.625f; a true division by 1.6f rounds differently for
+// about 15 % of fp32 scales (measured over every fp32 in [2^-14, 256) on an H100).
+#define DN_CHILD_SCALE (1.0f / 1.6f)
 
 struct PlaneToInt {
     const uint8_t *f;
@@ -58,7 +62,8 @@ k_densify_flags(int P, const float *__restrict__ accum, const float *__restrict_
     const bool faint = opa < min_opacity;                 // (:1026)
     const bool prune_orig = faint || (use_screen && smax > big_thr);   // (:1037-1040)
     // a child's scale is stored as log(s / (0.8 N)) (:949-951) and read back through exp (:110-111)
-    const float c0 = expf(logf(__fdiv_rn(s0, 1.6f))), c1 = expf(logf(__fdiv_rn(s1, 1.6f))), c2 = expf(logf(__fdiv_rn(s2, 1.6f)));
+    const float c0 = expf(logf(__fmul_rn(s0, DN_CHILD_SCALE))), c1 = expf(logf(__fmul_rn(s1, DN_CHILD_SCALE))),
+                c2 = expf(logf(__fmul_rn(s2, DN_CHILD_SCALE)));
     const bool prune_child = faint || (use_screen && fmaxf(c0, fmaxf(c1, c2)) > big_thr);
     flags[i] = (!sel_split && !prune_orig) ? 1 : 0;
     flags[(size_t)P + i] = (sel_clone && !prune_orig) ? 1 : 0;
@@ -78,8 +83,8 @@ __global__ void k_densify_totals(int P, const uint8_t *__restrict__ flags, const
 // counts_host (HOST, 6 int32): rows kept, clones, children copy 1, children copy 2, S = Gaussians selected for the split
 // (the split consumes 2 S rows of `noise`), and the new number of Gaussians.  Synchronises `stream`.
 extern "C" int gs_densify_select(int P, const float *xyz_gradient_accum, const float *denom, const float *scaling_raw,
-                                 const float *opacity_raw, float max_grad, float min_opacity, float extent,
-                                 float percent_dense, int use_screen_size, void *temp, size_t temp_bytes,
+                                 const float *opacity_raw, float max_grad, float min_opacity, double extent,
+                                 double percent_dense, int use_screen_size, void *temp, size_t temp_bytes,
                                  int32_t *counts_host, void *stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     GS_REQUIRE(P > 0, "P");
@@ -95,8 +100,9 @@ extern "C" int gs_densify_select(int P, const float *xyz_gradient_accum, const f
     int32_t *totals = (int32_t *)((char *)pos + dn_align(4 * n));
     void *scratch = (char *)totals + 256;
     size_t scratch_bytes = dn_scan_bytes(P);
-    // the thresholds are Python doubles in the reference, rounded to fp32 when compared with fp32 tensors
-    const float dense_thr = (float)((double)percent_dense * (double)extent), big_thr = (float)(0.1 * (double)extent);
+    // the thresholds are Python doubles in the reference (percent_dense * extent, 0.1 * extent), rounded to fp32 once
+    // when compared with fp32 tensors: form the product in double from the unrounded inputs, then round
+    const float dense_thr = (float)(percent_dense * extent), big_thr = (float)(0.1 * extent);
     k_densify_flags<<<(P + DN_THREADS - 1) / DN_THREADS, DN_THREADS, 0, stream>>>(
         P, xyz_gradient_accum, denom, scaling_raw, opacity_raw, max_grad, min_opacity, dense_thr, big_thr,
         use_screen_size ? 1 : 0, flags);
@@ -147,7 +153,7 @@ k_densify_gather(int P, int S, const DnTensors t, const float *__restrict__ scal
         if (kind == DN_MOMENT) {
             c[0] = c[1] = 0.f;
         } else if (kind == DN_SCALING) {
-            c[0] = c[1] = logf(__fdiv_rn(expf(v), 1.6f));       // scaling_inverse_activation(get_scaling / (0.8 N))
+            c[0] = c[1] = logf(__fmul_rn(expf(v), DN_CHILD_SCALE));   // scaling_inverse_activation(get_scaling / (0.8 N))
         } else if (kind == DN_XYZ) {
             // new_xyz = R(q) (s * z) + xyz, R of utils/general_utils.py:416-438 on the RAW quaternion
             const float q0 = rotation[4 * i], q1 = rotation[4 * i + 1], q2 = rotation[4 * i + 2], q3 = rotation[4 * i + 3];
@@ -193,7 +199,8 @@ extern "C" int gs_densify_gather(int P, int S, int new_P, int num_tensors, const
         t.width[k] = v ? width_host[k] : 0;
         t.kind[k] = v ? kind_host[k] : 0;
         if (!v) continue;
-        GS_REQUIRE(t.src[k] && t.dst[k] && t.width[k] > 0 && t.kind[k] >= DN_COPY && t.kind[k] <= DN_MOMENT, "tensor table");
+        // an output of new_P == 0 rows may have no storage (a NULL pointer): nothing is written to it
+        GS_REQUIRE(t.src[k] && (t.dst[k] || new_P == 0) && t.width[k] > 0 && t.kind[k] >= DN_COPY && t.kind[k] <= DN_MOMENT, "tensor table");
         GS_REQUIRE((t.kind[k] != DN_XYZ && t.kind[k] != DN_SCALING) || t.width[k] == 3, "position / scale rows have 3 elements");
         widest = t.width[k] > widest ? t.width[k] : widest;
     }

@@ -4,7 +4,7 @@
 // (/root/reference/train_internal.py:316-329; optimizer built at scene/gaussian_model.py:257-292, six groups,
 // eps 1e-15).  Arithmetic is torch.optim.Adam's (no weight decay, no amsgrad, maximize off), in its operation order:
 //     g      = grad * grad_scale
-//     m      = m + (1 - beta1) (g - m)                    (lerp)
+//     m      = m + (1 - beta1) (g - m)                    (lerp; g - (g - m) beta1 when 1 - beta1 >= 0.5)
 //     v      = v beta2 + (1 - beta2) g g                  (mul, addcmul)
 //     denom  = sqrt(v) / sqrt(1 - beta2^t) + eps
 //     p      = p - (lr / (1 - beta1^t)) m / denom         (addcdiv)
@@ -33,10 +33,12 @@ struct AdamTensors {
 GS_D void adam_one(float &p, float g, float &m, float &v, float gs, float w1, float beta2, float w2, float bc2_sqrt,
                    float eps, float step_size) {
     g = g * gs;
-    m = __fmaf_rn(w1, g - m, m);
+    // torch's lerp (ATen/native/Lerp.h): m + w (g - m) for |w| < 0.5, else g - (g - m) (1 - w)
+    m = w1 < 0.5f ? __fmaf_rn(w1, g - m, m) : __fmaf_rn(-(g - m), 1.f - w1, g);
     v = __fmaf_rn(w2, g * g, v * beta2);
-    const float denom = __fdiv_rn(__fsqrt_rn(v), bc2_sqrt) + eps;
-    p = p - step_size * __fdiv_rn(m, denom);
+    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), eps);
+    // addcdiv_(m, denom, value=-step_size) on CUDA is one fma: p + (-step_size) (m / denom), rounded once
+    p = __fmaf_rn(-step_size, __fdiv_rn(m, denom), p);
 }
 
 __global__ void __launch_bounds__(AD_THREADS)

@@ -14,6 +14,16 @@ LIB_PATH = os.environ.get("GS_B200_LIB") or os.path.join(_PKG, "lib", "libgrende
 
 _vp, _i, _f, _i64, _sz = C.c_void_p, C.c_int, C.c_float, C.c_int64, C.c_size_t
 
+
+class _real(C.c_double):
+    """A C double parameter that takes a Python number or a ctypes float / double object.  A c_float converts exactly
+    (its fp32 value), so callers written when the parameter was a float keep working and keep their values."""
+
+    @classmethod
+    def from_param(cls, obj):
+        return C.c_double(obj.value if isinstance(obj, (C.c_float, C.c_double)) else obj)
+
+
 # name -> (restype, argtypes); mirrors include/grendel_gs_b200.h declaration by declaration
 SIGNATURES = {
     "gs_last_error": (C.c_char_p, []),
@@ -70,7 +80,7 @@ SIGNATURES = {
     "gs_adam_step": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_float, _vp]),
     "gs_knn3_mean_dist2": (_i, [_i, _vp, _vp, _vp]),
     "gs_densify_temp_bytes": (_sz, [_i]),
-    "gs_densify_select": (_i, [_i, _vp, _vp, _vp, _vp, C.c_float, C.c_float, C.c_float, C.c_float, _i, _vp, _sz, _vp, _vp]),
+    "gs_densify_select": (_i, [_i, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _real, _real, _i, _vp, _sz, _vp, _vp]),
     "gs_densify_gather": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gs_peer_alloc": (_i, [_sz, C.POINTER(C.c_void_p), _vp]),
     "gs_peer_open": (_i, [_vp, C.POINTER(C.c_void_p)]),

@@ -6,8 +6,9 @@ three launches and one host read-back instead of ~150 torch kernels and a dozen 
 
 The optimizer is edited the way the reference edits it: every group gets a NEW nn.Parameter, its state entry moves to
 the new parameter with exp_avg / exp_avg_sq replaced (survivors keep their moments, new Gaussians start at zero) and
-"step" untouched.  No CPU path.  NOT yet run on a device (written after round 1's GPU budget was spent); the algorithm is
-checked on CPU against the reference's own run (tests/test_densify_oracle.py).
+"step" untouched.  No CPU path.  The algorithm is checked on CPU against the reference's own run
+(tests/test_densify_oracle.py) and on the device, decision for decision and bit for bit, against the reference's chain
+of torch operations run on the same device (tests/test_densify_gpu.py).
 """
 import ctypes as C
 
@@ -53,8 +54,8 @@ def densify_and_prune(optimizer, xyz_gradient_accum, denom, max_grad, min_opacit
     temp = torch.empty((tb,), dtype=torch.uint8, device=dev)
     counts = (C.c_int32 * 6)()
     _lib.call("gs_densify_select", P, accum.data_ptr(), den.data_ptr(), params["scaling"].data_ptr(),
-              params["opacity"].data_ptr(), C.c_float(max_grad), C.c_float(min_opacity), C.c_float(extent),
-              C.c_float(percent_dense), 1 if max_screen_size else 0, temp.data_ptr(), tb, counts, stream)
+              params["opacity"].data_ptr(), C.c_float(max_grad), C.c_float(min_opacity), C.c_double(extent),
+              C.c_double(percent_dense), 1 if max_screen_size else 0, temp.data_ptr(), tb, counts, stream)
     kept, clones, child1, child2, S, new_P = (int(c) for c in counts)
     if noise is None:
         noise = torch.randn((max(2 * S, 1), 3), dtype=torch.float32, device=dev)

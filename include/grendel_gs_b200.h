@@ -440,14 +440,16 @@ GS_API int gs_adam_step(int num_tensors, const int64_t *numel_host, void *const 
  * and ONE scan that yields the output row of every survivor / clone / split child (order of the reference's end state:
  * survivors, clones, children copy 1, children copy 2; each in index order) and reads six counts back;
  * gs_densify_gather then writes every tensor once (moments of new Gaussians zero, children: position
- * R(q)(s * z) + x from caller-provided standard-normal draws z, log-scale log(s / 1.6)).
+ * R(q)(s * z) + x from caller-provided standard-normal draws z, log-scale log(s * fl32(1 / 1.6)), the product torch
+ * forms for s / 1.6 on CUDA).
  * counts_host: HOST int32[6] = kept, clones, children copy 1, children copy 2, S (split-selected; the split reads
  * 2 S rows of noise), new number of Gaussians.  scaling_raw / opacity_raw / rotation_raw are the raw parameters
- * (log-scale, logit, unnormalised quaternion).  Written after round 1's device budget was spent: NOT yet run on a GPU. */
+ * (log-scale, logit, unnormalised quaternion).  extent and percent_dense are doubles, like the reference's Python
+ * floats: the thresholds are fl32(percent_dense * extent) and fl32(0.1 * extent), rounded once from the double product. */
 GS_API size_t gs_densify_temp_bytes(int P);
 GS_API int gs_densify_select(int P, const float *xyz_gradient_accum, const float *denom, const float *scaling_raw,
-                             const float *opacity_raw, float max_grad, float min_opacity, float extent,
-                             float percent_dense, int use_screen_size, void *temp, size_t temp_bytes,
+                             const float *opacity_raw, float max_grad, float min_opacity, double extent,
+                             double percent_dense, int use_screen_size, void *temp, size_t temp_bytes,
                              int32_t *counts_host, void *stream);
 /* src_host / dst_host: HOST arrays of num_tensors (<= 24) device pointers to (P, width) inputs / (new_P, width) outputs of
  * 4-byte elements; kind_host: 0 copy, 1 position (width 3), 2 log-scale (width 3), 3 Adam moment. */
