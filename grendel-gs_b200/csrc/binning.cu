@@ -18,6 +18,7 @@
 
 #include "common.cuh"
 #include <atomic>
+#include <cfloat>
 #include <mutex>
 
 #define BIN_THREADS 256
@@ -74,7 +75,9 @@ k_count_tiles(int P, int W, int H, const float *__restrict__ means2D, const floa
     const uint32_t n = my_n;
     const float2 m = *reinterpret_cast<const float2 *>(means2D + 2 * i);
     touched[i] = n;
-    depth_key[i] = n > 0 ? __float_as_uint(depths[i]) : 0xffffffffu;  // depths are > 0.2: bits sort like values
+    // raw bits, as the published 64-bit key: for positive depths they sort like the values; -0, negative depths and
+    // NaN sort after +inf, in bit order (tests/test_binning_gpu.py::test_depth_orders_bit_exact)
+    depth_key[i] = n > 0 ? __float_as_uint(depths[i]) : 0xffffffffu;
     index[i] = (uint32_t)i;
     float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f), r1 = r0, r2 = r0;
     if (n > 0) {
@@ -90,8 +93,10 @@ k_count_tiles(int P, int W, int H, const float *__restrict__ means2D, const floa
         float ex = -1.f, ey = -1.f;  // never contributes
         // t == 0 is a live splat: fl(1/255) is the one opacity whose 255 o rounds to exactly 1 (thr = -0), and it lies
         // above 1/255, so the pixel on its mean (power = +0) blends it -- as the alpha >= 1/255 test does
+        // a subnormal det has lost that accuracy (A = 4.2e-45, C = 0.5: det = 2.1e-45 rounds to 2.8e-45 and ey came
+        // out 1 % short of the true extent): below FLT_MIN the conic is treated as degenerate, never culled
         if (t >= 0.f) {
-            if (!no_cull && det > 0.f && co.x > 0.f && co.z > 0.f) {
+            if (!no_cull && det >= FLT_MIN && co.x > 0.f && co.z > 0.f) {
                 ex = sqrtf(t * co.z / det) * 1.02f + 0.5f;
                 ey = sqrtf(t * co.x / det) * 1.02f + 0.5f;
             } else {

@@ -159,7 +159,7 @@ GS_API int gs_render_count(int P, int image_height, int image_width, const float
 GS_API size_t gs_render_sort_temp_bytes(int64_t R);
 
 /* Bytes of the segment workspace that links a forward to its backward (R instances, num_tiles = tiles of all views):
- * the forward leaves a per-pixel checkpoint every 64 entries of a tile list plus the list of (tile, segment) units,
+ * the forward leaves a per-pixel checkpoint every 128 entries (SEG_K) of a tile list plus the list of (tile, segment) units,
  * which lets gs_render_backward walk every segment independently (csrc/blend.cu, k_blend_bwd_seg).  No reference
  * counterpart: the published backward re-walks each tile list as a whole (cuda_rasterizer/backward.cu). */
 GS_API size_t gs_render_seg_bytes(int64_t R, int num_tiles);
