@@ -622,11 +622,12 @@ extern "C" int gs_xchg_pack_grad_p2p(int nseg, const int32_t *seg_recv_start_hos
 // ---- sparse per-Gaussian gradient all-reduce staging (replicated-Gaussian data parallelism) ------------------
 // /root/reference/scene/gaussian_model.py:1332-1391 (get_sparse_ids / sync_gradients_sparsely): rows whose
 // _xyz.grad is non-zero on ANY rank are compacted, all-reduced and scattered back -- per parameter, i.e. 1 + 6
-// collectives and 12 gather/scatter kernels.  Here the six gradients of a touched Gaussian travel as ONE 59-float
-// row (xyz 3, features_dc 3, features_rest 45, scaling 3, rotation 4, opacity 1), so the step is: mask kernel ->
-// all-reduce(MAX) of the byte mask -> scan -> pack -> ONE all-reduce(SUM) -> unpack.  (The reference lists this
-// "fused_sparse" mode as NotImplemented, gaussian_model.py:1438-1439.)
-#define SG_FLOATS 59
+// collectives and 12 gather/scatter kernels.  Here the six gradients of a touched Gaussian travel as ONE row of
+// 14 + rest = 11 + 3 K floats (xyz 3, features_dc 3, features_rest rest = 3 (K - 1): 45 at the default max_sh_degree
+// 3, scaling 3, rotation 4, opacity 1), so the step is: mask kernel -> all-reduce(MAX) of the byte mask -> scan ->
+// pack -> ONE all-reduce(SUM) -> unpack.  (The reference lists this "fused_sparse" mode as NotImplemented,
+// gaussian_model.py:1438-1439.)
+#define SG_FIXED_FLOATS 14   // xyz, features_dc, scaling, rotation, opacity
 
 __global__ void __launch_bounds__(DT_THREADS)
 k_sparse_mask(int P, const float *__restrict__ xyz_grad, uint8_t *__restrict__ mask) {
@@ -648,12 +649,12 @@ struct SgPtrs { float *p[6]; };
 
 template <bool PACK>
 __global__ void __launch_bounds__(DT_THREADS)
-k_sparse_rows(int P, const uint8_t *__restrict__ mask, const int32_t *__restrict__ pos, SgPtrs g,
+k_sparse_rows(int P, int rest, const uint8_t *__restrict__ mask, const int32_t *__restrict__ pos, SgPtrs g,
               float *__restrict__ rows) {
     const int i = blockIdx.x * DT_THREADS + threadIdx.x;
     if (i >= P || !mask[i]) return;
-    float *r = rows + (size_t)pos[i] * SG_FLOATS;
-    const int width[6] = {3, 3, 45, 3, 4, 1};
+    float *r = rows + (size_t)pos[i] * (SG_FIXED_FLOATS + rest);
+    const int width[6] = {3, 3, rest, 3, 4, 1};
     int o = 0;
 #pragma unroll
     for (int t = 0; t < 6; t++) {
@@ -665,32 +666,46 @@ k_sparse_rows(int P, const uint8_t *__restrict__ mask, const int32_t *__restrict
     }
 }
 
-// grads_host: HOST array of the six device gradient pointers in GaussianModel order
-// (_xyz, _features_dc, _features_rest, _scaling, _rotation, _opacity); pos: exclusive scan of mask (gs_route_scan
-// with ncols = 1); rows: (n_touched, 59).
-extern "C" int gs_sparse_grad_pack(int P, const uint8_t *mask, const int32_t *pos, void *const *grads_host,
-                                   float *rows, void *stream) {
+template <bool PACK>
+static int sparse_rows(int P, int rest_floats, const uint8_t *mask, const int32_t *pos, void *const *grads_host,
+                       float *rows, void *stream) {
     GS_REQUIRE(P >= 0, "P");
+    GS_REQUIRE(rest_floats == 0 || rest_floats == 9 || rest_floats == 24 || rest_floats == 45,
+               "rest_floats must be 3 ((max_sh_degree + 1)^2 - 1): 0, 9, 24 or 45");
     if (P == 0) return GS_OK;
     GS_REQUIRE(mask && pos && grads_host && rows, "null pointer");
     SgPtrs g;
-    for (int t = 0; t < 6; t++) { g.p[t] = (float *)grads_host[t]; GS_REQUIRE(g.p[t] != nullptr, "null gradient"); }
-    k_sparse_rows<true><<<(P + DT_THREADS - 1) / DT_THREADS, DT_THREADS, 0, (cudaStream_t)stream>>>(P, mask, pos, g, rows);
+    for (int t = 0; t < 6; t++) {
+        g.p[t] = (float *)grads_host[t];
+        GS_REQUIRE(g.p[t] != nullptr || (t == 2 && rest_floats == 0), "null gradient");
+    }
+    k_sparse_rows<PACK><<<(P + DT_THREADS - 1) / DT_THREADS, DT_THREADS, 0, (cudaStream_t)stream>>>(
+        P, rest_floats, mask, pos, g, rows);
     GS_LAUNCH_CHECK();
     return GS_OK;
 }
 
+// grads_host: HOST array of the six device gradient pointers in GaussianModel order
+// (_xyz, _features_dc, _features_rest, _scaling, _rotation, _opacity); pos: exclusive scan of mask (gs_route_scan
+// with ncols = 1); rows: (n_touched, 14 + rest_floats).
+extern "C" int gs_sparse_grad_pack_rows(int P, int rest_floats, const uint8_t *mask, const int32_t *pos,
+                                        void *const *grads_host, float *rows, void *stream) {
+    return sparse_rows<true>(P, rest_floats, mask, pos, grads_host, rows, stream);
+}
+
+extern "C" int gs_sparse_grad_unpack_rows(int P, int rest_floats, const uint8_t *mask, const int32_t *pos,
+                                          const float *rows, void *const *grads_host, void *stream) {
+    return sparse_rows<false>(P, rest_floats, mask, pos, grads_host, const_cast<float *>(rows), stream);
+}
+
+extern "C" int gs_sparse_grad_pack(int P, const uint8_t *mask, const int32_t *pos, void *const *grads_host,
+                                   float *rows, void *stream) {
+    return gs_sparse_grad_pack_rows(P, 45, mask, pos, grads_host, rows, stream);
+}
+
 extern "C" int gs_sparse_grad_unpack(int P, const uint8_t *mask, const int32_t *pos, const float *rows,
                                      void *const *grads_host, void *stream) {
-    GS_REQUIRE(P >= 0, "P");
-    if (P == 0) return GS_OK;
-    GS_REQUIRE(mask && pos && grads_host && rows, "null pointer");
-    SgPtrs g;
-    for (int t = 0; t < 6; t++) { g.p[t] = (float *)grads_host[t]; GS_REQUIRE(g.p[t] != nullptr, "null gradient"); }
-    k_sparse_rows<false><<<(P + DT_THREADS - 1) / DT_THREADS, DT_THREADS, 0, (cudaStream_t)stream>>>(
-        P, mask, pos, g, const_cast<float *>(rows));
-    GS_LAUNCH_CHECK();
-    return GS_OK;
+    return gs_sparse_grad_unpack_rows(P, 45, mask, pos, rows, grads_host, stream);
 }
 
 // ---- direct-placement exchange (round 2) ---------------------------------------------------------------------------

@@ -1,23 +1,26 @@
 // Per-splat projection: stages "10 preprocess" / "b20 preprocess", the forward and backward of
 // GaussianRasterizer.preprocess_gaussians (gaussian_renderer/__init__.py:949-958 of the reference).  Three forms share
 // one set of stage functions:
-//   k_preprocess_{fwd,bwd}<false>   activated inputs, SH as one (P,16,3) block        gs_preprocess_{forward,backward}
-//   k_preprocess_{fwd,bwd}<true>    the six raw GaussianModel parameters, activations fused in          ..._raw
-//   k_preprocess_{fwd,bwd}_batched  raw parameters, all B cameras of a step per launch, each splat read once  ..._batched
+//   k_preprocess_{fwd,bwd}<false,K>   activated inputs, SH as one (P,K,3) block        gs_preprocess_{forward,backward}
+//   k_preprocess_{fwd,bwd}<true,K>    the six raw GaussianModel parameters, activations fused in          ..._raw
+//   k_preprocess_{fwd,bwd}_batched<K> raw parameters, all B cameras of a step per launch, each splat read once  ..._batched
+// K = (max_sh_degree + 1)^2 in {1, 4, 9, 16} is the number of SH coefficients the model stores (--sh_degree of the
+// reference, scene/gaussian_model.py:51-53, 150-156).  A K-coefficient kernel does the K = 16 kernel's fp32 operations
+// minus the terms whose basis value is zero (coefficients beyond the active degree), so with the stored coefficients
+// zero-padded to 16 both give the same bits.
 // Compiled with -fmad=false: radius, tile rectangle and depth key follow the IEEE fp32 operation sequence that
 // oracle/gs_oracle.c repeats, so tile indices are bit-exact; the kernels are HBM-bound, so losing FMA costs nothing.
-// A CTA's SH rows (192 B per splat) come into shared memory by TMA bulk copies issued before the projection math, and
+// A CTA's SH rows (12 K bytes per splat) come into shared memory by TMA bulk copies issued before the projection math, and
 // dL/dSH leaves by TMA bulk stores.  cams (batched): (B, 40) floats per camera: viewmatrix[16], projmatrix[16]
 // (transposed storage, scene/cameras.py:84-99), campos[3], tanfovx, tanfovy, 3 pad.
 #include <initializer_list>
+#include <type_traits>
 #include "common.cuh"
 
 #define PP_THREADS 128
 #define PB_BWD_THREADS 64
 #define PB_MAX_CAMS 64
-#define SH_FLOATS 48
 #define DC_FLOATS 3
-#define REST_FLOATS 45
 #define CAM_FLOATS 40
 
 static __device__ __constant__ float c_SH_C0 = 0.28209479177387814f;
@@ -73,39 +76,43 @@ GS_D void load_scale_rot(const float *scale, const float *rot, int i, float3 &sc
 }
 
 // ---- SH rows in shared memory ---------------------------------------------------------------------------------------
-// The CTA's SH rows (flat index f = 3 * coefficient + channel) lie in one block of 48 floats per splat or, SPLIT (the
-// raw parameters), in a block of the 3 dc floats per splat followed by a block of the 45 rest floats.
-template <bool SPLIT> constexpr int N0 = SPLIT ? DC_FLOATS : SH_FLOATS;  // floats per splat in the first block
+// The CTA's SH rows (flat index f = 3 * coefficient + channel, f < 3 K) lie in one block of 3 K floats per splat or,
+// SPLIT (the raw parameters), in a block of the 3 dc floats per splat followed by a block of the 3 (K - 1) rest floats
+// (none at K = 1: the rest pointers are then never read or written, and may be NULL).
+template <bool SPLIT, int K> constexpr int N0 = SPLIT ? DC_FLOATS : 3 * K;       // floats per splat in the first block
+template <bool SPLIT, int K> constexpr int N1 = SPLIT ? 3 * (K - 1) : 0;         // ... and in the rest block
 
-template <int THREADS, bool SPLIT>
+template <int THREADS, bool SPLIT, int K>
 struct ShRow {  // thread t's row
     float *s;
     int t;
     GS_D float &operator[](int f) const {
-        constexpr int n0 = N0<SPLIT>;
-        return f < n0 ? s[t * n0 + f] : s[THREADS * n0 + t * REST_FLOATS + (f - n0)];
+        constexpr int n0 = N0<SPLIT, K>;
+        return f < n0 ? s[t * n0 + f] : s[THREADS * n0 + t * N1<SPLIT, K> + (f - n0)];
     }
 };
 
 // Bring the rows of the CTA's nvalid splats into s_sh.  Returns true when they come by TMA on the mbarrier, false when
-// by plain loads: a bulk copy's size must be a multiple of 16 B, which a split ragged tail block misses when its splat
-// count is not a multiple of 4.
-template <int THREADS, bool SPLIT>
+// by plain loads: a bulk copy's size must be a multiple of 16 B, which a ragged tail block of n floats per splat misses
+// when n is not a multiple of 4 and its splat count is not a multiple of 4 (the dc block of the split forms, and the
+// unsplit block at K = 1 and K = 9).
+template <int THREADS, bool SPLIT, int K>
 GS_D bool stage_sh(float *s_sh, uint64_t *bar, const float *sh, const float *sh_rest, int base, int nvalid) {
-    constexpr int n0 = N0<SPLIT>;
+    constexpr int n0 = N0<SPLIT, K>, n1 = N1<SPLIT, K>;
     float *s_dc = s_sh, *s_rest = s_sh + THREADS * n0;
-    const bool tma = !SPLIT || (nvalid & 3) == 0;
+    const bool tma = (n0 % 4 == 0 && n1 % 4 == 0) || (nvalid & 3) == 0;
     if (threadIdx.x == 0) { gs_mbar_init(bar, 1); gs_fence_mbar_init(); }
     __syncthreads();
     if (tma) {
         if (threadIdx.x == 0) {
-            gs_mbar_arrive_expect_tx(bar, (uint32_t)nvalid * SH_FLOATS * 4u);
+            gs_mbar_arrive_expect_tx(bar, (uint32_t)nvalid * (n0 + n1) * 4u);
             gs_bulk_g2s(s_dc, sh + (size_t)base * n0, (uint32_t)nvalid * n0 * 4u, bar);
-            if (SPLIT) gs_bulk_g2s(s_rest, sh_rest + (size_t)base * REST_FLOATS, (uint32_t)nvalid * REST_FLOATS * 4u, bar);
+            if constexpr (n1 > 0) gs_bulk_g2s(s_rest, sh_rest + (size_t)base * n1, (uint32_t)nvalid * n1 * 4u, bar);
         }
     } else {
         for (int k = threadIdx.x; k < nvalid * n0; k += THREADS) s_dc[k] = sh[(size_t)base * n0 + k];
-        for (int k = threadIdx.x; k < nvalid * REST_FLOATS; k += THREADS) s_rest[k] = sh_rest[(size_t)base * REST_FLOATS + k];
+        if constexpr (n1 > 0)
+            for (int k = threadIdx.x; k < nvalid * n1; k += THREADS) s_rest[k] = sh_rest[(size_t)base * n1 + k];
     }
     return tma;
 }
@@ -114,22 +121,23 @@ GS_D bool stage_sh(float *s_sh, uint64_t *bar, const float *sh, const float *sh_
 GS_D void wait_sh(bool tma, uint64_t *bar) { if (tma) gs_mbar_wait(bar, 0); else __syncthreads(); }
 
 // Write the CTA's dL/dSH rows from s_sh to d_sh (and d_sh_rest): TMA bulk stores, or plain stores after plain loads.
-template <int THREADS, bool SPLIT>
+template <int THREADS, bool SPLIT, int K>
 GS_D void store_sh(float *d_sh, float *d_sh_rest, float *s_sh, bool tma, int base, int nvalid) {
-    constexpr int n0 = N0<SPLIT>;
+    constexpr int n0 = N0<SPLIT, K>, n1 = N1<SPLIT, K>;
     float *s_dc = s_sh, *s_rest = s_sh + THREADS * n0;
     gs_fence_proxy_async_smem();
     __syncthreads();
     if (tma) {
         if (threadIdx.x == 0) {
             gs_bulk_s2g(d_sh + (size_t)base * n0, s_dc, (uint32_t)nvalid * n0 * 4u);
-            if (SPLIT) gs_bulk_s2g(d_sh_rest + (size_t)base * REST_FLOATS, s_rest, (uint32_t)nvalid * REST_FLOATS * 4u);
+            if constexpr (n1 > 0) gs_bulk_s2g(d_sh_rest + (size_t)base * n1, s_rest, (uint32_t)nvalid * n1 * 4u);
             gs_bulk_commit();
             gs_bulk_wait_read0();
         }
     } else {
         for (int k = threadIdx.x; k < nvalid * n0; k += THREADS) d_sh[(size_t)base * n0 + k] = s_dc[k];
-        for (int k = threadIdx.x; k < nvalid * REST_FLOATS; k += THREADS) d_sh_rest[(size_t)base * REST_FLOATS + k] = s_rest[k];
+        if constexpr (n1 > 0)
+            for (int k = threadIdx.x; k < nvalid * n1; k += THREADS) d_sh_rest[(size_t)base * n1 + k] = s_rest[k];
     }
 }
 
@@ -263,8 +271,8 @@ GS_D float3 view_dir(const float3 p, const float *cp, float &len) {
 }
 
 // Colour of a visible splat: its SH of degree D along the view direction, + 0.5, clamped at 0.  cm gets the clamp
-// bits (1, 2, 4 = r, g, b) that mask the backward.
-template <class Row>
+// bits (1, 2, 4 = r, g, b) that mask the backward.  The row holds K coefficients, D <= sqrt(K) - 1.
+template <int K, class Row>
 GS_D float3 sh_forward(int D, const float3 p, const float *cp, const Row sh, uint8_t &cm) {
     float len;
     const float3 d = view_dir(p, cp, len);
@@ -272,7 +280,7 @@ GS_D float3 sh_forward(int D, const float3 p, const float *cp, const Row sh, uin
     sh_basis(D, d.x, d.y, d.z, bas);
     float acc[3] = {0.f, 0.f, 0.f};
 #pragma unroll
-    for (int f = 0; f < SH_FLOATS; f++) acc[f % 3] += bas[f / 3] * sh[f];
+    for (int f = 0; f < 3 * K; f++) acc[f % 3] += bas[f / 3] * sh[f];
     float c0 = acc[0] + 0.5f, c1 = acc[1] + 0.5f, c2 = acc[2] + 0.5f;
     cm = 0;
     if (c0 < 0.f) { cm |= 1; c0 = 0.f; }
@@ -380,8 +388,8 @@ GS_D void sigma_backward(const float G[6], const float4 q, const float3 sc, floa
 // Colour gradient g_rgb (3 floats; channels clamped in the forward get none) -> dL/dSH of the row and the gradient
 // through the view direction into the mean, which is returned.  ACCUM (several cameras): the dL/dSH of the
 // coefficients in use is added to row g.  Otherwise every slot of row sh is overwritten with its gradient (zero beyond
-// degree D) and g is not touched.
-template <bool ACCUM, class Row>
+// degree D) and g is not touched.  The rows hold K coefficients, D <= sqrt(K) - 1.
+template <bool ACCUM, int K, class Row>
 GS_D float3 sh_backward(int D, const float3 p, const float *cp, uint8_t cm, const float *g_rgb, const Row sh,
                         const Row g) {
     float len;
@@ -393,13 +401,15 @@ GS_D float3 sh_backward(int D, const float3 p, const float *cp, uint8_t cm, cons
     const int ncoef = (D + 1) * (D + 1);
     float s[16] = {};  // dL/d(basis value), per coefficient
 #pragma unroll
-    for (int j = 0; j < SH_FLOATS; j += 4) {
+    for (int j = 0; j < 3 * K; j += 4) {
         float v[4];  // four loads, then four stores: on a contiguous row both vectorise
 #pragma unroll
-        for (int e = 0; e < 4; e++) v[e] = sh[j + e];
+        for (int e = 0; e < 4; e++)
+            if (j + e < 3 * K) v[e] = sh[j + e];
 #pragma unroll
         for (int e = 0; e < 4; e++) {
             const int f = j + e, k = f / 3, ch = f % 3;
+            if (f >= 3 * K) break;
             if constexpr (ACCUM) {
                 if (k < ncoef) { s[k] += v[e] * dc[ch]; g[f] += bas[k] * dc[ch]; }
             } else {
@@ -437,19 +447,19 @@ GS_D float3 sh_backward(int D, const float3 p, const float *cp, uint8_t cm, cons
 }
 
 // ---- single-camera kernels ------------------------------------------------------------------------------------------
-// RAW = false: scale, rotation (unit), opacity as the rasterizer takes them and sh = the (P,16,3) block (sh_rest and
+// RAW = false: scale, rotation (unit), opacity as the rasterizer takes them and sh = the (P,K,3) block (sh_rest and
 // d_sh_rest unused).  RAW = true: the GaussianModel parameters, sh / sh_rest = _features_dc / _features_rest.
-template <bool RAW>
+template <bool RAW, int K>
 __global__ void __launch_bounds__(PP_THREADS) k_preprocess_fwd(
     int P, int D, const float *__restrict__ xyz, const float *__restrict__ sh, const float *__restrict__ sh_rest,
     const float *__restrict__ scale, float mod, const float *__restrict__ rot, const float *__restrict__ opac,
     const float *__restrict__ viewmatrix, const float *__restrict__ projmatrix, const float *__restrict__ campos,
     int W, int H, float tanfovx, float tanfovy, float *__restrict__ means2D, float *__restrict__ depths,
     int32_t *__restrict__ radii, float *__restrict__ conic_opacity, float *__restrict__ rgb, uint8_t *__restrict__ clamped) {
-    __shared__ __align__(128) float s_sh[PP_THREADS * SH_FLOATS];
+    __shared__ __align__(128) float s_sh[PP_THREADS * 3 * K];
     __shared__ __align__(8) uint64_t s_bar;
     const int base = blockIdx.x * PP_THREADS, nvalid = min(PP_THREADS, P - base);
-    const bool tma = stage_sh<PP_THREADS, RAW>(s_sh, &s_bar, sh, sh_rest, base, nvalid);
+    const bool tma = stage_sh<PP_THREADS, RAW, K>(s_sh, &s_bar, sh, sh_rest, base, nvalid);
     const int i = base + threadIdx.x;
     bool vis = false;
     Footprint fp = {};
@@ -473,11 +483,11 @@ __global__ void __launch_bounds__(PP_THREADS) k_preprocess_fwd(
     wait_sh(tma, &s_bar);
     if (i >= P) return;
     float3 c = make_float3(0.f, 0.f, 0.f); uint8_t cm = 0;
-    if (vis) c = sh_forward(D, p, cam.cp, ShRow<PP_THREADS, RAW>{s_sh, (int)threadIdx.x}, cm);
+    if (vis) c = sh_forward<K>(D, p, cam.cp, ShRow<PP_THREADS, RAW, K>{s_sh, (int)threadIdx.x}, cm);
     store_footprint(i, fp, c, cm, means2D, depths, radii, conic_opacity, rgb, clamped);
 }
 
-template <bool RAW>
+template <bool RAW, int K>
 __global__ void __launch_bounds__(PP_THREADS) k_preprocess_bwd(
     int P, int D, const float *__restrict__ xyz, const float *__restrict__ sh, const float *__restrict__ sh_rest,
     const float *__restrict__ scale, float mod, const float *__restrict__ rot, const float *__restrict__ opac,
@@ -486,10 +496,10 @@ __global__ void __launch_bounds__(PP_THREADS) k_preprocess_bwd(
     const float *__restrict__ g_means2D, const float *__restrict__ g_conic_opacity, const float *__restrict__ g_rgb,
     float *__restrict__ d_xyz, float *__restrict__ d_sh, float *__restrict__ d_sh_rest, float *__restrict__ d_scale,
     float *__restrict__ d_rot, float *__restrict__ d_opac) {
-    __shared__ __align__(128) float s_sh[PP_THREADS * SH_FLOATS];
+    __shared__ __align__(128) float s_sh[PP_THREADS * 3 * K];
     __shared__ __align__(8) uint64_t s_bar;
     const int base = blockIdx.x * PP_THREADS, nvalid = min(PP_THREADS, P - base);
-    const bool tma = stage_sh<PP_THREADS, RAW>(s_sh, &s_bar, sh, sh_rest, base, nvalid);
+    const bool tma = stage_sh<PP_THREADS, RAW, K>(s_sh, &s_bar, sh, sh_rest, base, nvalid);
     const int i = base + threadIdx.x;
     const bool act = (i < P) && (radii[i] > 0);
     float3 p = make_float3(0.f, 0.f, 0.f), gm = p, gs = p;
@@ -519,30 +529,31 @@ __global__ void __launch_bounds__(PP_THREADS) k_preprocess_bwd(
     wait_sh(tma, &s_bar);
     // colour -> SH coefficients (written in place over the staged rows) and view direction
     if (i < P) {
-        const ShRow<PP_THREADS, RAW> row{s_sh, (int)threadIdx.x};
+        const ShRow<PP_THREADS, RAW, K> row{s_sh, (int)threadIdx.x};
         if (act) {
-            gm = add3(gm, sh_backward<false>(D, p, cam.cp, clamped[i], g_rgb + 3 * i, row, row));
+            gm = add3(gm, sh_backward<false, K>(D, p, cam.cp, clamped[i], g_rgb + 3 * i, row, row));
         } else {
 #pragma unroll
-            for (int f = 0; f < SH_FLOATS; f++) row[f] = 0.f;
+            for (int f = 0; f < 3 * K; f++) row[f] = 0.f;
         }
         st3(d_xyz + 3 * i, gm); st3(d_scale + 3 * i, gs);
         *reinterpret_cast<float4 *>(d_rot + 4 * i) = gq;
         d_opac[i] = gop;
     }
-    store_sh<PP_THREADS, RAW>(d_sh, d_sh_rest, s_sh, tma, base, nvalid);
+    store_sh<PP_THREADS, RAW, K>(d_sh, d_sh_rest, s_sh, tma, base, nvalid);
 }
 
 // ---- batched kernels: B cameras, each Gaussian read once ------------------------------------------------------------
+template <int K>
 __global__ void __launch_bounds__(PP_THREADS) k_preprocess_fwd_batched(
     int B, int P, int D, const float *__restrict__ xyz, const float *__restrict__ f_dc, const float *__restrict__ f_rest,
     const float *__restrict__ scaling, float mod, const float *__restrict__ rotation, const float *__restrict__ opacity,
     const float *__restrict__ cams, int W, int H, float *__restrict__ means2D, float *__restrict__ depths,
     int32_t *__restrict__ radii, float *__restrict__ conic_opacity, float *__restrict__ rgb, uint8_t *__restrict__ clamped) {
-    __shared__ __align__(128) float s_sh[PP_THREADS * SH_FLOATS];
+    __shared__ __align__(128) float s_sh[PP_THREADS * 3 * K];
     __shared__ __align__(8) uint64_t s_bar;
     const int base = blockIdx.x * PP_THREADS, nvalid = min(PP_THREADS, P - base);
-    const bool tma = stage_sh<PP_THREADS, true>(s_sh, &s_bar, f_dc, f_rest, base, nvalid);
+    const bool tma = stage_sh<PP_THREADS, true, K>(s_sh, &s_bar, f_dc, f_rest, base, nvalid);
     const int i = base + threadIdx.x;
     float3 p = make_float3(0.f, 0.f, 0.f), sc = p;
     float4 q = make_float4(1.f, 0.f, 0.f, 0.f);
@@ -557,7 +568,7 @@ __global__ void __launch_bounds__(PP_THREADS) k_preprocess_fwd_batched(
     }
     wait_sh(tma, &s_bar);
     if (i >= P) return;
-    const ShRow<PP_THREADS, true> row{s_sh, (int)threadIdx.x};
+    const ShRow<PP_THREADS, true, K> row{s_sh, (int)threadIdx.x};
     for (int k = 0; k < B; k++) {
         Cam cam; float tanfovx, tanfovy;
         load_cam_row(cam, tanfovx, tanfovy, cams + (size_t)k * CAM_FLOATS);
@@ -566,12 +577,13 @@ __global__ void __launch_bounds__(PP_THREADS) k_preprocess_fwd_batched(
         float3 c = make_float3(0.f, 0.f, 0.f); uint8_t cm = 0;
         if (project<true>(cam, p, sc, mod, q, fx, fy, tanfovx, tanfovy, pr) && screen(pr, W, H, fp)) {
             fp.co.w = op;
-            c = sh_forward(D, p, cam.cp, row, cm);
+            c = sh_forward<K>(D, p, cam.cp, row, cm);
         }
         store_footprint((size_t)k * P + i, fp, c, cm, means2D, depths, radii, conic_opacity, rgb, clamped);
     }
 }
 
+template <int K>
 __global__ void __launch_bounds__(PB_BWD_THREADS) k_preprocess_bwd_batched(
     int B, int P, int D, const float *__restrict__ xyz, const float *__restrict__ f_dc, const float *__restrict__ f_rest,
     const float *__restrict__ scaling, float mod, const float *__restrict__ rotation, const float *__restrict__ opacity,
@@ -579,15 +591,15 @@ __global__ void __launch_bounds__(PB_BWD_THREADS) k_preprocess_bwd_batched(
     const float *__restrict__ g_means2D, const float *__restrict__ g_conic_opacity, const float *__restrict__ g_rgb,
     float *__restrict__ d_xyz, float *__restrict__ d_dc, float *__restrict__ d_rest, float *__restrict__ d_scaling,
     float *__restrict__ d_rotation, float *__restrict__ d_opacity) {
-    __shared__ __align__(128) float s_sh[PB_BWD_THREADS * SH_FLOATS];   // SH coefficients of the CTA's splats
-    __shared__ __align__(128) float s_g[PB_BWD_THREADS * SH_FLOATS];    // dL/dSH accumulated over the cameras
+    __shared__ __align__(128) float s_sh[PB_BWD_THREADS * 3 * K];   // SH coefficients of the CTA's splats
+    __shared__ __align__(128) float s_g[PB_BWD_THREADS * 3 * K];    // dL/dSH accumulated over the cameras
     __shared__ __align__(8) uint64_t s_bar;
     const int base = blockIdx.x * PB_BWD_THREADS, nvalid = min(PB_BWD_THREADS, P - base);
-    const bool tma = stage_sh<PB_BWD_THREADS, true>(s_sh, &s_bar, f_dc, f_rest, base, nvalid);
+    const bool tma = stage_sh<PB_BWD_THREADS, true, K>(s_sh, &s_bar, f_dc, f_rest, base, nvalid);
     const int i = base + threadIdx.x;
-    const ShRow<PB_BWD_THREADS, true> row{s_sh, (int)threadIdx.x}, grow{s_g, (int)threadIdx.x};
+    const ShRow<PB_BWD_THREADS, true, K> row{s_sh, (int)threadIdx.x}, grow{s_g, (int)threadIdx.x};
 #pragma unroll
-    for (int f = 0; f < SH_FLOATS; f++) grow[f] = 0.f;
+    for (int f = 0; f < 3 * K; f++) grow[f] = 0.f;
     float3 p = make_float3(0.f, 0.f, 0.f), sc = p;
     float4 q = make_float4(1.f, 0.f, 0.f, 0.f);
     float den = 1.f, op = 0.f;
@@ -615,7 +627,7 @@ __global__ void __launch_bounds__(PB_BWD_THREADS) k_preprocess_bwd_batched(
             gm = add3(add3(gm, cg.m_cov), cg.m_2d);
 #pragma unroll
             for (int e = 0; e < 6; e++) G[e] += cg.G[e];
-            gm = add3(gm, sh_backward<true>(D, p, cam.cp, clamped[o], g_rgb + 3 * o, row, grow));
+            gm = add3(gm, sh_backward<true, K>(D, p, cam.cp, clamped[o], g_rgb + 3 * o, row, grow));
         }
         // Sigma -> (scale, rotation) once, with the accumulated dL/dSigma
         float3 gs; float4 dq;
@@ -625,21 +637,29 @@ __global__ void __launch_bounds__(PB_BWD_THREADS) k_preprocess_bwd_batched(
         *reinterpret_cast<float4 *>(d_rotation + 4 * i) = normalize4_backward(q, dq, den);
         d_opacity[i] = gop * op * (1.f - op);  // sigmoid'
     }
-    store_sh<PB_BWD_THREADS, true>(d_dc, d_rest, s_g, tma, base, nvalid);
+    store_sh<PB_BWD_THREADS, true, K>(d_dc, d_rest, s_g, tma, base, nvalid);
 }
 
 // ---- C ABI ----------------------------------------------------------------------------------------------------------
 // Checks shared by the entry points: GS_EINVAL with the error set, or GS_OK.  B is the camera count (1 for the
-// single-camera forms).  With P == 0 nothing past the sizes is checked, and launch() does nothing.
-static int check_args(int B, int P, int sh_degree, bool image_ok, std::initializer_list<const void *> ptrs,
-                      std::initializer_list<const void *> aligned16, const void *aligned8) {
+// single-camera forms).  rest: the features_rest pointers of the split forms, unused (and allowed to be NULL) when the
+// model stores degree 0 only.  With P == 0 nothing past the sizes is checked, and launch() does nothing.
+static int check_args(int B, int P, int sh_degree, int max_sh_degree, bool image_ok,
+                      std::initializer_list<const void *> ptrs, std::initializer_list<const void *> aligned16,
+                      const void *aligned8, std::initializer_list<const void *> rest = {}) {
     GS_REQUIRE(B > 0 && B <= PB_MAX_CAMS && P >= 0, "sizes");
-    GS_REQUIRE(sh_degree >= 0 && sh_degree <= 3, "sh_degree must be 0..3");
+    GS_REQUIRE(max_sh_degree >= 0 && max_sh_degree <= 3, "max_sh_degree must be 0..3");
+    GS_REQUIRE(sh_degree >= 0 && sh_degree <= max_sh_degree, "sh_degree must be 0..max_sh_degree");
     if (P == 0) return GS_OK;
     GS_REQUIRE(image_ok, "image size");
     for (const void *p : ptrs) GS_REQUIRE(p != nullptr, "null pointer");
     for (const void *p : aligned16) GS_REQUIRE(((uintptr_t)p & 15) == 0, "16-byte alignment");
     GS_REQUIRE(((uintptr_t)aligned8 & 7) == 0, "8-byte alignment");
+    if (max_sh_degree > 0)
+        for (const void *p : rest) {
+            GS_REQUIRE(p != nullptr, "null features_rest pointer with max_sh_degree > 0");
+            GS_REQUIRE(((uintptr_t)p & 15) == 0, "16-byte alignment");
+        }
     return GS_OK;
 }
 
@@ -652,19 +672,62 @@ static int launch(int stage, int P, int threads, void *stream, void (*kernel)(Pa
     return GS_OK;
 }
 
+// f(std::integral_constant<int, K>) with K = (max_sh_degree + 1)^2, the instantiation for the stored coefficients
+template <class F>
+static int with_coefficients(int max_sh_degree, F f) {
+    switch (max_sh_degree) {
+    case 0: return f(std::integral_constant<int, 1>{});
+    case 1: return f(std::integral_constant<int, 4>{});
+    case 2: return f(std::integral_constant<int, 9>{});
+    default: return f(std::integral_constant<int, 16>{});
+    }
+}
+
+extern "C" int gs_preprocess_forward_sh(
+    int P, int sh_degree, int max_sh_degree, const float *means3D, const float *scales, float scale_modifier,
+    const float *rotations, const float *opacities, const float *shs, const float *viewmatrix, const float *projmatrix,
+    const float *campos, int image_width, int image_height, float tanfovx, float tanfovy, float *means2D, float *depths,
+    int32_t *radii, float *conic_opacity, float *rgb, uint8_t *clamped, void *stream) {
+    // unlike the other entry points, this one has always refused an empty image even when P == 0
+    GS_REQUIRE(image_width > 0 && image_height > 0, "image size");
+    if (int rc = check_args(1, P, sh_degree, max_sh_degree, true, {means3D, scales, rotations, opacities, shs,
+                            viewmatrix, projmatrix, campos, means2D, depths, radii, conic_opacity, rgb, clamped},
+                            {shs, rotations, conic_opacity}, means2D)) return rc;
+    return with_coefficients(max_sh_degree, [&](auto k) {
+        return launch(GS_STAGE_PREPROCESS_FWD, P, PP_THREADS, stream, k_preprocess_fwd<false, decltype(k)::value>, P,
+                      sh_degree, means3D, shs, (const float *)nullptr, scales, scale_modifier, rotations, opacities,
+                      viewmatrix, projmatrix, campos, image_width, image_height, tanfovx, tanfovy, means2D, depths,
+                      radii, conic_opacity, rgb, clamped);
+    });
+}
+
 extern "C" int gs_preprocess_forward(
     int P, int sh_degree, const float *means3D, const float *scales, float scale_modifier, const float *rotations,
     const float *opacities, const float *shs, const float *viewmatrix, const float *projmatrix, const float *campos,
     int image_width, int image_height, float tanfovx, float tanfovy, float *means2D, float *depths, int32_t *radii,
     float *conic_opacity, float *rgb, uint8_t *clamped, void *stream) {
-    // unlike the other entry points, this one has always refused an empty image even when P == 0
-    GS_REQUIRE(image_width > 0 && image_height > 0, "image size");
-    if (int rc = check_args(1, P, sh_degree, true, {means3D, scales, rotations, opacities, shs, viewmatrix, projmatrix,
-                            campos, means2D, depths, radii, conic_opacity, rgb, clamped},
-                            {shs, rotations, conic_opacity}, means2D)) return rc;
-    return launch(GS_STAGE_PREPROCESS_FWD, P, PP_THREADS, stream, k_preprocess_fwd<false>, P, sh_degree, means3D, shs,
-                  nullptr, scales, scale_modifier, rotations, opacities, viewmatrix, projmatrix, campos, image_width,
-                  image_height, tanfovx, tanfovy, means2D, depths, radii, conic_opacity, rgb, clamped);
+    return gs_preprocess_forward_sh(P, sh_degree, 3, means3D, scales, scale_modifier, rotations, opacities, shs,
+                                    viewmatrix, projmatrix, campos, image_width, image_height, tanfovx, tanfovy, means2D,
+                                    depths, radii, conic_opacity, rgb, clamped, stream);
+}
+
+extern "C" int gs_preprocess_backward_sh(
+    int P, int sh_degree, int max_sh_degree, const float *means3D, const float *scales, float scale_modifier,
+    const float *rotations, const float *shs, const float *viewmatrix, const float *projmatrix, const float *campos,
+    int image_width, int image_height, float tanfovx, float tanfovy, const int32_t *radii, const uint8_t *clamped,
+    const float *dL_dmeans2D, const float *dL_dconic_opacity, const float *dL_drgb, float *dL_dmeans3D,
+    float *dL_dscales, float *dL_drotations, float *dL_dopacities, float *dL_dshs, void *stream) {
+    if (int rc = check_args(1, P, sh_degree, max_sh_degree, true, {means3D, scales, rotations, shs, viewmatrix,
+                            projmatrix, campos, radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dmeans3D,
+                            dL_dscales, dL_drotations, dL_dopacities, dL_dshs},
+                            {shs, dL_dshs, rotations, dL_drotations, dL_dconic_opacity}, dL_dmeans2D)) return rc;
+    return with_coefficients(max_sh_degree, [&](auto k) {
+        return launch(GS_STAGE_PREPROCESS_BWD, P, PP_THREADS, stream, k_preprocess_bwd<false, decltype(k)::value>, P,
+                      sh_degree, means3D, shs, (const float *)nullptr, scales, scale_modifier, rotations,
+                      (const float *)nullptr, viewmatrix, projmatrix, campos, image_width, image_height, tanfovx,
+                      tanfovy, radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dmeans3D, dL_dshs,
+                      (float *)nullptr, dL_dscales, dL_drotations, dL_dopacities);
+    });
 }
 
 extern "C" int gs_preprocess_backward(
@@ -673,14 +736,27 @@ extern "C" int gs_preprocess_backward(
     int image_height, float tanfovx, float tanfovy, const int32_t *radii, const uint8_t *clamped,
     const float *dL_dmeans2D, const float *dL_dconic_opacity, const float *dL_drgb, float *dL_dmeans3D,
     float *dL_dscales, float *dL_drotations, float *dL_dopacities, float *dL_dshs, void *stream) {
-    if (int rc = check_args(1, P, sh_degree, true, {means3D, scales, rotations, shs, viewmatrix, projmatrix, campos,
-                            radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dmeans3D, dL_dscales,
-                            dL_drotations, dL_dopacities, dL_dshs},
-                            {shs, dL_dshs, rotations, dL_drotations, dL_dconic_opacity}, dL_dmeans2D)) return rc;
-    return launch(GS_STAGE_PREPROCESS_BWD, P, PP_THREADS, stream, k_preprocess_bwd<false>, P, sh_degree, means3D, shs,
-                  nullptr, scales, scale_modifier, rotations, nullptr, viewmatrix, projmatrix, campos, image_width,
-                  image_height, tanfovx, tanfovy, radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dmeans3D,
-                  dL_dshs, nullptr, dL_dscales, dL_drotations, dL_dopacities);
+    return gs_preprocess_backward_sh(P, sh_degree, 3, means3D, scales, scale_modifier, rotations, shs, viewmatrix,
+                                     projmatrix, campos, image_width, image_height, tanfovx, tanfovy, radii, clamped,
+                                     dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dmeans3D, dL_dscales, dL_drotations,
+                                     dL_dopacities, dL_dshs, stream);
+}
+
+extern "C" int gs_preprocess_forward_raw_sh(
+    int P, int sh_degree, int max_sh_degree, const float *xyz, const float *features_dc, const float *features_rest,
+    const float *scaling, float scale_modifier, const float *rotation, const float *opacity, const float *viewmatrix,
+    const float *projmatrix, const float *campos, int image_width, int image_height, float tanfovx, float tanfovy,
+    float *means2D, float *depths, int32_t *radii, float *conic_opacity, float *rgb, uint8_t *clamped, void *stream) {
+    if (int rc = check_args(1, P, sh_degree, max_sh_degree, image_width > 0 && image_height > 0, {xyz, features_dc,
+                            scaling, rotation, opacity, viewmatrix, projmatrix, campos, means2D, depths, radii,
+                            conic_opacity, rgb, clamped},
+                            {features_dc, rotation, conic_opacity}, means2D, {features_rest})) return rc;
+    return with_coefficients(max_sh_degree, [&](auto k) {
+        return launch(GS_STAGE_PREPROCESS_FWD, P, PP_THREADS, stream, k_preprocess_fwd<true, decltype(k)::value>, P,
+                      sh_degree, xyz, features_dc, features_rest, scaling, scale_modifier, rotation, opacity,
+                      viewmatrix, projmatrix, campos, image_width, image_height, tanfovx, tanfovy, means2D, depths,
+                      radii, conic_opacity, rgb, clamped);
+    });
 }
 
 extern "C" int gs_preprocess_forward_raw(
@@ -688,13 +764,30 @@ extern "C" int gs_preprocess_forward_raw(
     float scale_modifier, const float *rotation, const float *opacity, const float *viewmatrix, const float *projmatrix,
     const float *campos, int image_width, int image_height, float tanfovx, float tanfovy, float *means2D, float *depths,
     int32_t *radii, float *conic_opacity, float *rgb, uint8_t *clamped, void *stream) {
-    if (int rc = check_args(1, P, sh_degree, image_width > 0 && image_height > 0, {xyz, features_dc, features_rest,
-                            scaling, rotation, opacity, viewmatrix, projmatrix, campos, means2D, depths, radii,
-                            conic_opacity, rgb, clamped},
-                            {features_dc, features_rest, rotation, conic_opacity}, means2D)) return rc;
-    return launch(GS_STAGE_PREPROCESS_FWD, P, PP_THREADS, stream, k_preprocess_fwd<true>, P, sh_degree, xyz, features_dc,
-                  features_rest, scaling, scale_modifier, rotation, opacity, viewmatrix, projmatrix, campos,
-                  image_width, image_height, tanfovx, tanfovy, means2D, depths, radii, conic_opacity, rgb, clamped);
+    return gs_preprocess_forward_raw_sh(P, sh_degree, 3, xyz, features_dc, features_rest, scaling, scale_modifier,
+                                        rotation, opacity, viewmatrix, projmatrix, campos, image_width, image_height,
+                                        tanfovx, tanfovy, means2D, depths, radii, conic_opacity, rgb, clamped, stream);
+}
+
+extern "C" int gs_preprocess_backward_raw_sh(
+    int P, int sh_degree, int max_sh_degree, const float *xyz, const float *features_dc, const float *features_rest,
+    const float *scaling, float scale_modifier, const float *rotation, const float *opacity, const float *viewmatrix,
+    const float *projmatrix, const float *campos, int image_width, int image_height, float tanfovx, float tanfovy,
+    const int32_t *radii, const uint8_t *clamped, const float *dL_dmeans2D, const float *dL_dconic_opacity,
+    const float *dL_drgb, float *dL_dxyz, float *dL_dfeatures_dc, float *dL_dfeatures_rest, float *dL_dscaling,
+    float *dL_drotation, float *dL_dopacity, void *stream) {
+    if (int rc = check_args(1, P, sh_degree, max_sh_degree, true, {xyz, features_dc, scaling, rotation, opacity,
+                            viewmatrix, projmatrix, campos, radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb,
+                            dL_dxyz, dL_dfeatures_dc, dL_dscaling, dL_drotation, dL_dopacity},
+                            {features_dc, dL_dfeatures_dc, rotation, dL_drotation, dL_dconic_opacity}, dL_dmeans2D,
+                            {features_rest, dL_dfeatures_rest})) return rc;
+    return with_coefficients(max_sh_degree, [&](auto k) {
+        return launch(GS_STAGE_PREPROCESS_BWD, P, PP_THREADS, stream, k_preprocess_bwd<true, decltype(k)::value>, P,
+                      sh_degree, xyz, features_dc, features_rest, scaling, scale_modifier, rotation, opacity,
+                      viewmatrix, projmatrix, campos, image_width, image_height, tanfovx, tanfovy, radii, clamped,
+                      dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dxyz, dL_dfeatures_dc, dL_dfeatures_rest,
+                      dL_dscaling, dL_drotation, dL_dopacity);
+    });
 }
 
 extern "C" int gs_preprocess_backward_raw(
@@ -704,15 +797,26 @@ extern "C" int gs_preprocess_backward_raw(
     const uint8_t *clamped, const float *dL_dmeans2D, const float *dL_dconic_opacity, const float *dL_drgb,
     float *dL_dxyz, float *dL_dfeatures_dc, float *dL_dfeatures_rest, float *dL_dscaling, float *dL_drotation,
     float *dL_dopacity, void *stream) {
-    if (int rc = check_args(1, P, sh_degree, true, {xyz, features_dc, features_rest, scaling, rotation, opacity,
-                            viewmatrix, projmatrix, campos, radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb,
-                            dL_dxyz, dL_dfeatures_dc, dL_dfeatures_rest, dL_dscaling, dL_drotation, dL_dopacity},
-                            {features_dc, features_rest, dL_dfeatures_dc, dL_dfeatures_rest, rotation, dL_drotation,
-                             dL_dconic_opacity}, dL_dmeans2D)) return rc;
-    return launch(GS_STAGE_PREPROCESS_BWD, P, PP_THREADS, stream, k_preprocess_bwd<true>, P, sh_degree, xyz, features_dc,
-                  features_rest, scaling, scale_modifier, rotation, opacity, viewmatrix, projmatrix, campos,
-                  image_width, image_height, tanfovx, tanfovy, radii, clamped, dL_dmeans2D, dL_dconic_opacity,
-                  dL_drgb, dL_dxyz, dL_dfeatures_dc, dL_dfeatures_rest, dL_dscaling, dL_drotation, dL_dopacity);
+    return gs_preprocess_backward_raw_sh(P, sh_degree, 3, xyz, features_dc, features_rest, scaling, scale_modifier,
+                                         rotation, opacity, viewmatrix, projmatrix, campos, image_width, image_height,
+                                         tanfovx, tanfovy, radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb,
+                                         dL_dxyz, dL_dfeatures_dc, dL_dfeatures_rest, dL_dscaling, dL_drotation,
+                                         dL_dopacity, stream);
+}
+
+extern "C" int gs_preprocess_forward_batched_sh(
+    int B, int P, int sh_degree, int max_sh_degree, const float *xyz, const float *features_dc,
+    const float *features_rest, const float *scaling, float scale_modifier, const float *rotation,
+    const float *opacity, const float *cams, int image_width, int image_height, float *means2D, float *depths,
+    int32_t *radii, float *conic_opacity, float *rgb, uint8_t *clamped, void *stream) {
+    if (int rc = check_args(B, P, sh_degree, max_sh_degree, image_width > 0 && image_height > 0, {xyz, features_dc,
+                            scaling, rotation, opacity, cams, means2D, depths, radii, conic_opacity, rgb, clamped},
+                            {features_dc, rotation, conic_opacity}, means2D, {features_rest})) return rc;
+    return with_coefficients(max_sh_degree, [&](auto k) {
+        return launch(GS_STAGE_PREPROCESS_FWD, P, PP_THREADS, stream, k_preprocess_fwd_batched<decltype(k)::value>, B,
+                      P, sh_degree, xyz, features_dc, features_rest, scaling, scale_modifier, rotation, opacity, cams,
+                      image_width, image_height, means2D, depths, radii, conic_opacity, rgb, clamped);
+    });
 }
 
 extern "C" int gs_preprocess_forward_batched(
@@ -720,12 +824,29 @@ extern "C" int gs_preprocess_forward_batched(
     const float *scaling, float scale_modifier, const float *rotation, const float *opacity, const float *cams,
     int image_width, int image_height, float *means2D, float *depths, int32_t *radii, float *conic_opacity,
     float *rgb, uint8_t *clamped, void *stream) {
-    if (int rc = check_args(B, P, sh_degree, image_width > 0 && image_height > 0, {xyz, features_dc, features_rest,
-                            scaling, rotation, opacity, cams, means2D, depths, radii, conic_opacity, rgb, clamped},
-                            {features_dc, features_rest, rotation, conic_opacity}, means2D)) return rc;
-    return launch(GS_STAGE_PREPROCESS_FWD, P, PP_THREADS, stream, k_preprocess_fwd_batched, B, P, sh_degree, xyz,
-                  features_dc, features_rest, scaling, scale_modifier, rotation, opacity, cams, image_width,
-                  image_height, means2D, depths, radii, conic_opacity, rgb, clamped);
+    return gs_preprocess_forward_batched_sh(B, P, sh_degree, 3, xyz, features_dc, features_rest, scaling,
+                                            scale_modifier, rotation, opacity, cams, image_width, image_height,
+                                            means2D, depths, radii, conic_opacity, rgb, clamped, stream);
+}
+
+extern "C" int gs_preprocess_backward_batched_sh(
+    int B, int P, int sh_degree, int max_sh_degree, const float *xyz, const float *features_dc,
+    const float *features_rest, const float *scaling, float scale_modifier, const float *rotation,
+    const float *opacity, const float *cams, int image_width, int image_height, const int32_t *radii,
+    const uint8_t *clamped, const float *dL_dmeans2D, const float *dL_dconic_opacity, const float *dL_drgb,
+    float *dL_dxyz, float *dL_dfeatures_dc, float *dL_dfeatures_rest, float *dL_dscaling, float *dL_drotation,
+    float *dL_dopacity, void *stream) {
+    if (int rc = check_args(B, P, sh_degree, max_sh_degree, true, {xyz, features_dc, scaling, rotation, opacity, cams,
+                            radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dxyz, dL_dfeatures_dc,
+                            dL_dscaling, dL_drotation, dL_dopacity},
+                            {features_dc, dL_dfeatures_dc, rotation, dL_drotation, dL_dconic_opacity}, dL_dmeans2D,
+                            {features_rest, dL_dfeatures_rest})) return rc;
+    return with_coefficients(max_sh_degree, [&](auto k) {
+        return launch(GS_STAGE_PREPROCESS_BWD, P, PB_BWD_THREADS, stream, k_preprocess_bwd_batched<decltype(k)::value>,
+                      B, P, sh_degree, xyz, features_dc, features_rest, scaling, scale_modifier, rotation, opacity,
+                      cams, image_width, image_height, radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dxyz,
+                      dL_dfeatures_dc, dL_dfeatures_rest, dL_dscaling, dL_drotation, dL_dopacity);
+    });
 }
 
 extern "C" int gs_preprocess_backward_batched(
@@ -734,13 +855,9 @@ extern "C" int gs_preprocess_backward_batched(
     int image_width, int image_height, const int32_t *radii, const uint8_t *clamped, const float *dL_dmeans2D,
     const float *dL_dconic_opacity, const float *dL_drgb, float *dL_dxyz, float *dL_dfeatures_dc,
     float *dL_dfeatures_rest, float *dL_dscaling, float *dL_drotation, float *dL_dopacity, void *stream) {
-    if (int rc = check_args(B, P, sh_degree, true, {xyz, features_dc, features_rest, scaling, rotation, opacity, cams,
-                            radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dxyz, dL_dfeatures_dc,
-                            dL_dfeatures_rest, dL_dscaling, dL_drotation, dL_dopacity},
-                            {features_dc, features_rest, dL_dfeatures_dc, dL_dfeatures_rest, rotation, dL_drotation,
-                             dL_dconic_opacity}, dL_dmeans2D)) return rc;
-    return launch(GS_STAGE_PREPROCESS_BWD, P, PB_BWD_THREADS, stream, k_preprocess_bwd_batched, B, P, sh_degree, xyz,
-                  features_dc, features_rest, scaling, scale_modifier, rotation, opacity, cams, image_width,
-                  image_height, radii, clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dxyz, dL_dfeatures_dc,
-                  dL_dfeatures_rest, dL_dscaling, dL_drotation, dL_dopacity);
+    return gs_preprocess_backward_batched_sh(B, P, sh_degree, 3, xyz, features_dc, features_rest, scaling,
+                                             scale_modifier, rotation, opacity, cams, image_width, image_height, radii,
+                                             clamped, dL_dmeans2D, dL_dconic_opacity, dL_drgb, dL_dxyz,
+                                             dL_dfeatures_dc, dL_dfeatures_rest, dL_dscaling, dL_drotation,
+                                             dL_dopacity, stream);
 }

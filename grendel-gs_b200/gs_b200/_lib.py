@@ -41,6 +41,18 @@ SIGNATURES = {
                                            _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gs_preprocess_backward_batched": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _vp, _vp,
                                             _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_preprocess_forward_sh": (_i, [_i, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _f,
+                                      _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_preprocess_backward_sh": (_i, [_i, _i, _i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _f, _vp, _vp,
+                                       _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_preprocess_forward_raw_sh": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _f,
+                                          _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_preprocess_backward_raw_sh": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _f,
+                                           _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_preprocess_forward_batched_sh": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i,
+                                              _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_preprocess_backward_batched_sh": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _i, _vp,
+                                               _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gs_get_local2j_ids_bool": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "gs_get_local2j_ids_bool_rects": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "gs_render_count_temp_bytes": (_sz, [_i]),
@@ -96,6 +108,8 @@ SIGNATURES = {
     "gs_sparse_grad_mask": (_i, [_i, _vp, _vp, _vp]),
     "gs_sparse_grad_pack": (_i, [_i, _vp, _vp, _vp, _vp, _vp]),
     "gs_sparse_grad_unpack": (_i, [_i, _vp, _vp, _vp, _vp, _vp]),
+    "gs_sparse_grad_pack_rows": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "gs_sparse_grad_unpack_rows": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp]),
     "gs_get_touched_locally": (_i, [_i, _i, _i, _vp, _vp, _vp]),
     "gs_get_pixels_compute_locally_and_in_rect": (_i, [_i, _i, _vp, _i, _i, _i, _i, _vp, _vp]),
     "gs_image_tiles_gather": (_i, [_i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),

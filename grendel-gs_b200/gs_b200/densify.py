@@ -68,8 +68,10 @@ def densify_and_prune(optimizer, xyz_gradient_accum, denom, max_grad, min_opacit
     def add(name, t, k):
         t, w = _as_rows(t)
         o = torch.empty((new_P,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
-        src.append(t); dst.append(o); width.append(w); kind.append(k)
         outs[name] = o
+        if w == 0:   # _features_rest of a model stored at SH degree 0 (P,0,3): nothing to gather
+            return
+        src.append(t); dst.append(o); width.append(w); kind.append(k)
 
     with torch.no_grad():
         for k in NAMES:

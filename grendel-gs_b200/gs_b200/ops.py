@@ -106,6 +106,22 @@ def _screen_outputs(lead, dev):
             torch.empty((*lead, 3), dtype=f32, device=dev), torch.empty(lead, dtype=torch.uint8, device=dev))
 
 
+# stored SH coefficients K -> max_sh_degree: the reference's --sh_degree D keeps (D+1)^2 coefficients per Gaussian
+# (scene/gaussian_model.py:51-53, 150-156)
+_STORED_DEGREE = {1: 0, 4: 1, 9: 2, 16: 3}
+
+
+def _stored_degree(K, sh_degree, what):
+    """max_sh_degree of a model storing K SH coefficients; ValueError (before any launch) for any other K or for an active
+    sh_degree outside 0..max_sh_degree."""
+    if K not in _STORED_DEGREE:
+        raise ValueError(f"{what}: a model stores (D+1)^2 SH coefficients, D = 0..3 (1, 4, 9 or 16), got {K}")
+    D = _STORED_DEGREE[K]
+    if not 0 <= int(sh_degree) <= D:
+        raise ValueError(f"active sh_degree {sh_degree} is outside 0..{D}, the degree the model stores ({K} coefficients)")
+    return D
+
+
 def _grad_or_zeros(g, shape, dev):
     """An incoming gradient as contiguous fp32, or zeros where autograd passes None for an unused output."""
     return torch.zeros(shape, dtype=torch.float32, device=dev) if g is None else _f32c(g, "grad")
@@ -118,20 +134,21 @@ class _PreprocessGaussians(torch.autograd.Function):
         means3D, scales, rotations = _f32c(means3D, "means3D"), _f32c(scales, "scales"), _f32c(rotations, "rotations")
         shs, opacities = _f32c(shs, "shs"), _f32c(opacities, "opacities")
         P = means3D.shape[0]
-        if shs.dim() != 3 or shs.shape[1] != 16 or shs.shape[2] != 3:
-            raise ValueError(f"shs must be (P,16,3) (scene/gaussian_model.py:122-125), got {tuple(shs.shape)}")
+        if shs.dim() != 3 or shs.shape[2] != 3:
+            raise ValueError(f"shs must be (P,K,3) (scene/gaussian_model.py:122-125), got {tuple(shs.shape)}")
+        max_deg = _stored_degree(shs.shape[1], rs.sh_degree, "shs")
         if tuple(means3D.shape) != (P, 3) or tuple(scales.shape) != (P, 3) or tuple(rotations.shape) != (P, 4) \
                 or opacities.numel() != P or shs.shape[0] != P:
             raise ValueError("inconsistent Gaussian parameter shapes")
         dev = means3D.device
         vm, pm, cp = _f32c(rs.viewmatrix, "viewmatrix"), _f32c(rs.projmatrix, "projmatrix"), _f32c(rs.campos, "campos")
         means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((P,), dev)
-        _lib.call("gs_preprocess_forward", P, int(rs.sh_degree), means3D.data_ptr(), scales.data_ptr(),
+        _lib.call("gs_preprocess_forward_sh", P, int(rs.sh_degree), max_deg, means3D.data_ptr(), scales.data_ptr(),
                   float(rs.scale_modifier), rotations.data_ptr(), opacities.data_ptr(), shs.data_ptr(), vm.data_ptr(),
                   pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
                   float(rs.tanfovy), means2D.data_ptr(), depths.data_ptr(), radii.data_ptr(), conic_opacity.data_ptr(),
                   rgb.data_ptr(), clamped.data_ptr(), _stream())
-        ctx.rs = rs
+        ctx.rs, ctx.max_deg = rs, max_deg
         ctx.cam = (vm, pm, cp)
         ctx.save_for_backward(means3D, scales, rotations, shs, radii, clamped)
         ctx.mark_non_differentiable(radii, depths)
@@ -150,18 +167,19 @@ class _PreprocessGaussians(torch.autograd.Function):
         d_scales = torch.empty((P, 3), dtype=torch.float32, device=dev)
         d_rot = torch.empty((P, 4), dtype=torch.float32, device=dev)
         d_opac = torch.empty((P, 1), dtype=torch.float32, device=dev)
-        d_shs = torch.empty((P, 16, 3), dtype=torch.float32, device=dev)
-        _lib.call("gs_preprocess_backward", P, int(rs.sh_degree), means3D.data_ptr(), scales.data_ptr(),
-                  float(rs.scale_modifier), rotations.data_ptr(), shs.data_ptr(), vm.data_ptr(), pm.data_ptr(),
-                  cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx), float(rs.tanfovy),
-                  radii.data_ptr(), clamped.data_ptr(), g_means2D.data_ptr(), g_conic_opacity.data_ptr(),
-                  g_rgb.data_ptr(), d_means3D.data_ptr(), d_scales.data_ptr(), d_rot.data_ptr(), d_opac.data_ptr(),
-                  d_shs.data_ptr(), _stream())
+        d_shs = torch.empty(tuple(shs.shape), dtype=torch.float32, device=dev)
+        _lib.call("gs_preprocess_backward_sh", P, int(rs.sh_degree), ctx.max_deg, means3D.data_ptr(),
+                  scales.data_ptr(), float(rs.scale_modifier), rotations.data_ptr(), shs.data_ptr(), vm.data_ptr(),
+                  pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
+                  float(rs.tanfovy), radii.data_ptr(), clamped.data_ptr(), g_means2D.data_ptr(),
+                  g_conic_opacity.data_ptr(), g_rgb.data_ptr(), d_means3D.data_ptr(), d_scales.data_ptr(),
+                  d_rot.data_ptr(), d_opac.data_ptr(), d_shs.data_ptr(), _stream())
         return d_means3D, d_scales, d_rot, d_shs, d_opac, None
 
 
 def preprocess_gaussians(means3D, scales, rotations, shs, opacities, raster_settings, cuda_args=None):
-    """-> (means2D (P,2) pixels, rgb (P,3), conic_opacity (P,4), radii (P) int32, depths (P))."""
+    """-> (means2D (P,2) pixels, rgb (P,3), conic_opacity (P,4), radii (P) int32, depths (P)).
+    shs (P,K,3): the K = (D+1)^2 coefficients of a model stored at degree D = 0..3; raster_settings.sh_degree <= D."""
     return _PreprocessGaussians.apply(means3D, scales, rotations, shs, opacities, raster_settings)
 
 
@@ -174,20 +192,21 @@ class _PreprocessGaussiansRaw(torch.autograd.Function):
         xyz, f_dc, f_rest = _f32c(xyz, "_xyz"), _f32c(f_dc, "_features_dc"), _f32c(f_rest, "_features_rest")
         scaling, rotation, opacity = _f32c(scaling, "_scaling"), _f32c(rotation, "_rotation"), _f32c(opacity, "_opacity")
         P = xyz.shape[0]
-        if tuple(f_dc.shape) != (P, 1, 3) or tuple(f_rest.shape) != (P, 15, 3):
-            raise ValueError("features must be (P,1,3) and (P,15,3) (scene/gaussian_model.py:219-228)")
+        if tuple(f_dc.shape) != (P, 1, 3) or f_rest.dim() != 3 or f_rest.shape[0] != P or f_rest.shape[2] != 3:
+            raise ValueError("features must be (P,1,3) and (P,K-1,3) (scene/gaussian_model.py:219-228)")
+        max_deg = _stored_degree(f_rest.shape[1] + 1, rs.sh_degree, "_features_dc + _features_rest")
         if tuple(xyz.shape) != (P, 3) or tuple(scaling.shape) != (P, 3) or tuple(rotation.shape) != (P, 4) \
                 or opacity.numel() != P:
             raise ValueError("inconsistent Gaussian parameter shapes")
         dev = xyz.device
         vm, pm, cp = _f32c(rs.viewmatrix, "viewmatrix"), _f32c(rs.projmatrix, "projmatrix"), _f32c(rs.campos, "campos")
         means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((P,), dev)
-        _lib.call("gs_preprocess_forward_raw", P, int(rs.sh_degree), xyz.data_ptr(), f_dc.data_ptr(), f_rest.data_ptr(),
-                  scaling.data_ptr(), float(rs.scale_modifier), rotation.data_ptr(), opacity.data_ptr(), vm.data_ptr(),
-                  pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
-                  float(rs.tanfovy), means2D.data_ptr(), depths.data_ptr(), radii.data_ptr(), conic_opacity.data_ptr(),
-                  rgb.data_ptr(), clamped.data_ptr(), _stream())
-        ctx.rs = rs
+        _lib.call("gs_preprocess_forward_raw_sh", P, int(rs.sh_degree), max_deg, xyz.data_ptr(), f_dc.data_ptr(),
+                  f_rest.data_ptr(), scaling.data_ptr(), float(rs.scale_modifier), rotation.data_ptr(),
+                  opacity.data_ptr(), vm.data_ptr(), pm.data_ptr(), cp.data_ptr(), int(rs.image_width),
+                  int(rs.image_height), float(rs.tanfovx), float(rs.tanfovy), means2D.data_ptr(), depths.data_ptr(),
+                  radii.data_ptr(), conic_opacity.data_ptr(), rgb.data_ptr(), clamped.data_ptr(), _stream())
+        ctx.rs, ctx.max_deg = rs, max_deg
         ctx.cam = (vm, pm, cp)
         ctx.save_for_backward(xyz, f_dc, f_rest, scaling, rotation, opacity, radii, clamped)
         ctx.mark_non_differentiable(radii, depths)
@@ -203,18 +222,19 @@ class _PreprocessGaussiansRaw(torch.autograd.Function):
         g_means2D, g_rgb = _grad_or_zeros(g_means2D, (P, 2), dev), _grad_or_zeros(g_rgb, (P, 3), dev)
         g_conic_opacity = _grad_or_zeros(g_conic_opacity, (P, 4), dev)
         d = [torch.empty_like(t) for t in (xyz, f_dc, f_rest, scaling, rotation, opacity)]
-        _lib.call("gs_preprocess_backward_raw", P, int(rs.sh_degree), xyz.data_ptr(), f_dc.data_ptr(), f_rest.data_ptr(),
-                  scaling.data_ptr(), float(rs.scale_modifier), rotation.data_ptr(), opacity.data_ptr(), vm.data_ptr(),
-                  pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
-                  float(rs.tanfovy), radii.data_ptr(), clamped.data_ptr(), g_means2D.data_ptr(),
-                  g_conic_opacity.data_ptr(), g_rgb.data_ptr(), d[0].data_ptr(), d[1].data_ptr(), d[2].data_ptr(),
-                  d[3].data_ptr(), d[4].data_ptr(), d[5].data_ptr(), _stream())
+        _lib.call("gs_preprocess_backward_raw_sh", P, int(rs.sh_degree), ctx.max_deg, xyz.data_ptr(), f_dc.data_ptr(),
+                  f_rest.data_ptr(), scaling.data_ptr(), float(rs.scale_modifier), rotation.data_ptr(),
+                  opacity.data_ptr(), vm.data_ptr(), pm.data_ptr(), cp.data_ptr(), int(rs.image_width),
+                  int(rs.image_height), float(rs.tanfovx), float(rs.tanfovy), radii.data_ptr(), clamped.data_ptr(),
+                  g_means2D.data_ptr(), g_conic_opacity.data_ptr(), g_rgb.data_ptr(), d[0].data_ptr(), d[1].data_ptr(),
+                  d[2].data_ptr(), d[3].data_ptr(), d[4].data_ptr(), d[5].data_ptr(), _stream())
         return d[0], d[1], d[2], d[3], d[4], d[5], None
 
 
 def preprocess_gaussians_raw(xyz, features_dc, features_rest, scaling, rotation, opacity, raster_settings):
     """Same outputs as preprocess_gaussians, from the six RAW GaussianModel parameters
-    (scene/gaussian_model.py:219-228); the activations of :109-129 run inside the kernel."""
+    (scene/gaussian_model.py:219-228); the activations of :109-129 run inside the kernel.  features_rest (P,K-1,3),
+    (P,0,3) for a model stored at degree 0."""
     return _PreprocessGaussiansRaw.apply(xyz, features_dc, features_rest, scaling, rotation, opacity, raster_settings)
 
 
@@ -816,16 +836,18 @@ class _PreprocessBatched(torch.autograd.Function):
         scaling, rotation, opacity = _f32c(scaling, "_scaling"), _f32c(rotation, "_rotation"), _f32c(opacity, "_opacity")
         cams = _f32c(cams, "cams")
         P, B = xyz.shape[0], cams.shape[0]
-        if tuple(f_dc.shape) != (P, 1, 3) or tuple(f_rest.shape) != (P, 15, 3) or cams.shape[1] != 40:
-            raise ValueError("features must be (P,1,3)/(P,15,3) and cams (B,40)")
+        if tuple(f_dc.shape) != (P, 1, 3) or f_rest.dim() != 3 or f_rest.shape[0] != P or f_rest.shape[2] != 3 \
+                or cams.shape[1] != 40:
+            raise ValueError("features must be (P,1,3)/(P,K-1,3) and cams (B,40)")
         W, H, D, mod = meta
+        max_deg = _stored_degree(f_rest.shape[1] + 1, D, "_features_dc + _features_rest")
         dev = xyz.device
         means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((B, P), dev)
-        _lib.call("gs_preprocess_forward_batched", B, P, int(D), xyz.data_ptr(), f_dc.data_ptr(), f_rest.data_ptr(),
-                  scaling.data_ptr(), float(mod), rotation.data_ptr(), opacity.data_ptr(), cams.data_ptr(), int(W),
-                  int(H), means2D.data_ptr(), depths.data_ptr(), radii.data_ptr(), conic_opacity.data_ptr(),
-                  rgb.data_ptr(), clamped.data_ptr(), _stream())
-        ctx.meta = meta
+        _lib.call("gs_preprocess_forward_batched_sh", B, P, int(D), max_deg, xyz.data_ptr(), f_dc.data_ptr(),
+                  f_rest.data_ptr(), scaling.data_ptr(), float(mod), rotation.data_ptr(), opacity.data_ptr(),
+                  cams.data_ptr(), int(W), int(H), means2D.data_ptr(), depths.data_ptr(), radii.data_ptr(),
+                  conic_opacity.data_ptr(), rgb.data_ptr(), clamped.data_ptr(), _stream())
+        ctx.meta, ctx.max_deg = meta, max_deg
         ctx.save_for_backward(xyz, f_dc, f_rest, scaling, rotation, opacity, cams, radii, clamped)
         ctx.mark_non_differentiable(radii, depths)
         return means2D, rgb, conic_opacity, radii, depths
@@ -839,17 +861,18 @@ class _PreprocessBatched(torch.autograd.Function):
         g_means2D, g_rgb = _grad_or_zeros(g_means2D, (B, P, 2), dev), _grad_or_zeros(g_rgb, (B, P, 3), dev)
         g_conic_opacity = _grad_or_zeros(g_conic_opacity, (B, P, 4), dev)
         d = [torch.empty_like(t) for t in (xyz, f_dc, f_rest, scaling, rotation, opacity)]
-        _lib.call("gs_preprocess_backward_batched", B, P, int(D), xyz.data_ptr(), f_dc.data_ptr(), f_rest.data_ptr(),
-                  scaling.data_ptr(), float(mod), rotation.data_ptr(), opacity.data_ptr(), cams.data_ptr(), int(W),
-                  int(H), radii.data_ptr(), clamped.data_ptr(), g_means2D.data_ptr(), g_conic_opacity.data_ptr(),
-                  g_rgb.data_ptr(), d[0].data_ptr(), d[1].data_ptr(), d[2].data_ptr(), d[3].data_ptr(), d[4].data_ptr(),
-                  d[5].data_ptr(), _stream())
+        _lib.call("gs_preprocess_backward_batched_sh", B, P, int(D), ctx.max_deg, xyz.data_ptr(), f_dc.data_ptr(),
+                  f_rest.data_ptr(), scaling.data_ptr(), float(mod), rotation.data_ptr(), opacity.data_ptr(),
+                  cams.data_ptr(), int(W), int(H), radii.data_ptr(), clamped.data_ptr(), g_means2D.data_ptr(),
+                  g_conic_opacity.data_ptr(), g_rgb.data_ptr(), d[0].data_ptr(), d[1].data_ptr(), d[2].data_ptr(),
+                  d[3].data_ptr(), d[4].data_ptr(), d[5].data_ptr(), _stream())
         return d[0], d[1], d[2], d[3], d[4], d[5], None, None
 
 
 def preprocess_gaussians_batched(xyz, features_dc, features_rest, scaling, rotation, opacity, cams, image_width,
                                  image_height, sh_degree, scale_modifier=1.0):
-    """All B cameras at once from the RAW GaussianModel parameters.  cams: pack_cameras(...) (B,40).
+    """All B cameras at once from the RAW GaussianModel parameters (features_rest (P,K-1,3) as in
+    preprocess_gaussians_raw).  cams: pack_cameras(...) (B,40).
     -> (means2D (B,P,2), rgb (B,P,3), conic_opacity (B,P,4), radii (B,P) int32, depths (B,P)); slice k equals the
     single-camera operator's output for camera k."""
     return _PreprocessBatched.apply(xyz, features_dc, features_rest, scaling, rotation, opacity, cams,

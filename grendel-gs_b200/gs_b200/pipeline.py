@@ -51,12 +51,20 @@ class DeviceCamera:
 
 class GaussianParams(nn.Module):
     """The six raw nn.Parameter tensors of GaussianModel (scene/gaussian_model.py:219-228) with its
-    activations (:109-129).  Built from an ACTIVATED synthetic scene by inverting the activations."""
+    activations (:109-129).  Built from an ACTIVATED synthetic scene by inverting the activations.
+    max_sh_degree: the SH degree the model stores (--sh_degree, gaussian_model.py:51-53): the first (D+1)^2 coefficients
+    of scene["shs"] are kept, _features_rest is (P,(D+1)^2-1,3) (:150-156); active_sh_degree starts at it."""
 
-    def __init__(self, scene, device):
+    def __init__(self, scene, device, max_sh_degree=3):
         super().__init__()
+        if not 0 <= int(max_sh_degree) <= 3:
+            raise ValueError(f"max_sh_degree must be 0..3, got {max_sh_degree}")
+        K = (int(max_sh_degree) + 1) ** 2
+        if scene["shs"].shape[1] < K:
+            raise ValueError(f"the scene stores {scene['shs'].shape[1]} SH coefficients, max_sh_degree "
+                             f"{max_sh_degree} needs {K}")
         t = lambda a: torch.as_tensor(a, dtype=torch.float32).to(device)
-        shs = t(scene["shs"])
+        shs = t(scene["shs"][:, :K])
         op = t(scene["opacities"]).clamp(1e-6, 1 - 1e-6)
         self._xyz = nn.Parameter(t(scene["means3D"]).contiguous())
         # own storage, not views of shs: with one Gaussian shs[:, 1:, :] is already contiguous, so .contiguous() would
@@ -66,7 +74,8 @@ class GaussianParams(nn.Module):
         self._scaling = nn.Parameter(torch.log(t(scene["scales"])).contiguous())
         self._rotation = nn.Parameter(t(scene["rotations"]).contiguous())
         self._opacity = nn.Parameter(torch.log(op / (1 - op)).contiguous())
-        self.active_sh_degree = 3
+        self.max_sh_degree = int(max_sh_degree)
+        self.active_sh_degree = self.max_sh_degree
 
     @property
     def get_xyz(self):
@@ -117,7 +126,7 @@ class Trainer:
     def __init__(self, scene, cams, gts_pinned, device, rank=0, world=1, lambda_dssim=0.2, group=None,
                  fused_activations=True, border_exchange=False, batched_render=True, peer_exchange=None,
                  peer_cap_rows=None, shard=None, load_balance=True, heuristic_decay=0.0,
-                 distributed_dataset_storage=False, feedback_lag=None):
+                 distributed_dataset_storage=False, feedback_lag=None, max_sh_degree=3):
         """scene: the WHOLE scene (sliced here into this rank's contiguous shard), or -- shard=(lo, hi, n_total) -- only
         this rank's Gaussians [lo, hi) of an n_total-Gaussian scene (synthetic.make_scene_shard).
         load_balance: feed the measured render times back into the strip division after every step
@@ -129,7 +138,8 @@ class Trainer:
         read, all-gathered and applied before the next step starts, so the host waits for the device at the end of every
         step and cannot enqueue ahead).  > 0 (default 2, GS_B200_FEEDBACK_LAG) = the times of the step `feedback_lag`
         steps back, whose events have long completed, ride on the NEXT exchange's size all-gather (exchange.PIGGYBACK_IN):
-        no collective of their own, no host sync; the strips move the same way, `feedback_lag` steps later."""
+        no collective of their own, no host sync; the strips move the same way, `feedback_lag` steps later.
+        max_sh_degree: the SH degree the model stores (GaussianParams)."""
         from . import exchange as _ex
         self._ex = _ex
         # splat / gradient rows travel by direct NVLink stores from the pack kernels (exchange.PeerBuffers) instead of
@@ -162,12 +172,12 @@ class Trainer:
         self.border_exchange = border_exchange   # legacy row L1: exchange 5 halo rows so strip losses sum to the full-image loss
         if shard is None:
             lo, hi = n * rank // world, n * (rank + 1) // world
-            self.params = GaussianParams({k: v[lo:hi] for k, v in scene.items()}, device)
+            self.params = GaussianParams({k: v[lo:hi] for k, v in scene.items()}, device, max_sh_degree)
         else:
             lo, hi = int(shard[0]), int(shard[1])
             if scene["means3D"].shape[0] != hi - lo:
                 raise ValueError("shard=(lo, hi, n_total) does not match the scene passed")
-            self.params = GaussianParams(scene, device)
+            self.params = GaussianParams(scene, device, max_sh_degree)
         self.n_local, self.n_total = hi - lo, n
         self.load_balance, self.heuristic_decay = load_balance, heuristic_decay
         if feedback_lag is None:

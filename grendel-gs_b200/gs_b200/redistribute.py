@@ -67,7 +67,7 @@ def redistribute(optimizer, destination=None, group=None, generator=None):
                 tensors += [st["exp_avg"], st["exp_avg_sq"]]
         widths = [int(np.prod(t.shape[1:])) if t.dim() > 1 else 1 for t in tensors]
         order = torch.sort(destination, stable=True).indices
-        send = torch.cat([t.reshape(P, -1) for t in tensors], dim=1).index_select(0, order).contiguous()
+        send = torch.cat([t.reshape(P, w) for t, w in zip(tensors, widths)], dim=1).index_select(0, order).contiguous()
         n_new = int(sum(recv_splits))
         recv = torch.empty((n_new, send.shape[1]), dtype=send.dtype, device=dev)
         all_to_all_single(recv, send, recv_splits, send_splits, group)

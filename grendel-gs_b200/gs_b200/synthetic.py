@@ -70,10 +70,11 @@ def make_camera(width, height, fovx_deg=60.0, yaw_deg=0.0, sh_degree=3, uid=0):
                 campos=np.ascontiguousarray(campos), sh_degree=int(sh_degree))
 
 
-def make_scene(n, width, height, fovx_deg=60.0, seed=0, radius_px=6.0):
+def make_scene(n, width, height, fovx_deg=60.0, seed=0, radius_px=6.0, max_sh_degree=3):
     """n Gaussians in the activated parameterisation the operator receives
     (scene/gaussian_model.py:109-129: exp'd scales, normalised wxyz, sigmoid'd opacity,
-    SH (n,16,3) = cat(dc, rest))."""
+    SH (n,K,3) = cat(dc, rest), K = (max_sh_degree+1)^2).  A lower max_sh_degree draws the same scene and keeps the first
+    K coefficients."""
     rng = np.random.default_rng(seed)
     tanx = math.tan(math.radians(fovx_deg) / 2)
     tany = tanx * height / width
@@ -91,7 +92,9 @@ def make_scene(n, width, height, fovx_deg=60.0, seed=0, radius_px=6.0):
     rotations = (q / np.linalg.norm(q, axis=1, keepdims=True)).astype(np.float32)
     opacities = (1.0 / (1.0 + np.exp(-rng.normal(0.0, 1.5, (n, 1))))).astype(np.float32)
     shs = np.concatenate([rng.normal(0.0, 1.0, (n, 1, 3)), rng.normal(0.0, 0.1, (n, 15, 3))], 1).astype(np.float32)
-    return dict(means3D=means3D, scales=scales, rotations=rotations, opacities=opacities, shs=shs)
+    K = (int(max_sh_degree) + 1) ** 2
+    return dict(means3D=means3D, scales=scales, rotations=rotations, opacities=opacities,
+                shs=np.ascontiguousarray(shs[:, :K]))
 
 
 SHARD_CHUNK = 1 << 20

@@ -121,6 +121,62 @@ GS_API int gs_preprocess_backward_batched(int B, int P, int sh_degree, const flo
                                           float *dL_dfeatures_dc, float *dL_dfeatures_rest, float *dL_dscaling,
                                           float *dL_drotation, float *dL_dopacity, void *stream);
 
+/* The six preprocess forms for a model that stores fewer SH coefficients: the reference's --sh_degree D sets
+ * GaussianModel.max_sh_degree (0..3; README.md:235, arguments/__init__.py:87, scene/gaussian_model.py:51-53), the model
+ * then holds _features_dc (P,1,3) and _features_rest (P,K-1,3) with K = (D+1)^2 (gaussian_model.py:150-156, 219-225),
+ * and get_features hands the rasterizer their concatenation (P,K,3) (:122-125).  Same arguments as the entry point
+ * without the _sh suffix, plus max_sh_degree after sh_degree: shs / dL_dshs are (P,K,3), features_rest /
+ * dL_dfeatures_rest (P,K-1,3).  Requires 0 <= sh_degree <= max_sh_degree <= 3 (sh_degree is the active degree,
+ * oneupSHdegree, :136-138).  At max_sh_degree 0 there is no rest block: features_rest / dL_dfeatures_rest are neither
+ * read nor written and may be NULL.  The entry points without the suffix are these with max_sh_degree = 3.  With the
+ * stored coefficients zero-padded to 16, the max_sh_degree = 3 call gives the same bits in every output, and the first K
+ * coefficients of its dL/dSH. */
+GS_API int gs_preprocess_forward_sh(int P, int sh_degree, int max_sh_degree, const float *means3D, const float *scales,
+                                    float scale_modifier, const float *rotations, const float *opacities,
+                                    const float *shs, const float *viewmatrix, const float *projmatrix,
+                                    const float *campos, int image_width, int image_height, float tanfovx,
+                                    float tanfovy, float *means2D, float *depths, int32_t *radii, float *conic_opacity,
+                                    float *rgb, uint8_t *clamped, void *stream);
+GS_API int gs_preprocess_backward_sh(int P, int sh_degree, int max_sh_degree, const float *means3D, const float *scales,
+                                     float scale_modifier, const float *rotations, const float *shs,
+                                     const float *viewmatrix, const float *projmatrix, const float *campos,
+                                     int image_width, int image_height, float tanfovx, float tanfovy,
+                                     const int32_t *radii, const uint8_t *clamped, const float *dL_dmeans2D,
+                                     const float *dL_dconic_opacity, const float *dL_drgb, float *dL_dmeans3D,
+                                     float *dL_dscales, float *dL_drotations, float *dL_dopacities, float *dL_dshs,
+                                     void *stream);
+GS_API int gs_preprocess_forward_raw_sh(int P, int sh_degree, int max_sh_degree, const float *xyz,
+                                        const float *features_dc, const float *features_rest, const float *scaling,
+                                        float scale_modifier, const float *rotation, const float *opacity,
+                                        const float *viewmatrix, const float *projmatrix, const float *campos,
+                                        int image_width, int image_height, float tanfovx, float tanfovy,
+                                        float *means2D, float *depths, int32_t *radii, float *conic_opacity,
+                                        float *rgb, uint8_t *clamped, void *stream);
+GS_API int gs_preprocess_backward_raw_sh(int P, int sh_degree, int max_sh_degree, const float *xyz,
+                                         const float *features_dc, const float *features_rest, const float *scaling,
+                                         float scale_modifier, const float *rotation, const float *opacity,
+                                         const float *viewmatrix, const float *projmatrix, const float *campos,
+                                         int image_width, int image_height, float tanfovx, float tanfovy,
+                                         const int32_t *radii, const uint8_t *clamped, const float *dL_dmeans2D,
+                                         const float *dL_dconic_opacity, const float *dL_drgb, float *dL_dxyz,
+                                         float *dL_dfeatures_dc, float *dL_dfeatures_rest, float *dL_dscaling,
+                                         float *dL_drotation, float *dL_dopacity, void *stream);
+GS_API int gs_preprocess_forward_batched_sh(int B, int P, int sh_degree, int max_sh_degree, const float *xyz,
+                                            const float *features_dc, const float *features_rest,
+                                            const float *scaling, float scale_modifier, const float *rotation,
+                                            const float *opacity, const float *cams, int image_width,
+                                            int image_height, float *means2D, float *depths, int32_t *radii,
+                                            float *conic_opacity, float *rgb, uint8_t *clamped, void *stream);
+GS_API int gs_preprocess_backward_batched_sh(int B, int P, int sh_degree, int max_sh_degree, const float *xyz,
+                                             const float *features_dc, const float *features_rest,
+                                             const float *scaling, float scale_modifier, const float *rotation,
+                                             const float *opacity, const float *cams, int image_width,
+                                             int image_height, const int32_t *radii, const uint8_t *clamped,
+                                             const float *dL_dmeans2D, const float *dL_dconic_opacity,
+                                             const float *dL_drgb, float *dL_dxyz, float *dL_dfeatures_dc,
+                                             float *dL_dfeatures_rest, float *dL_dscaling, float *dL_drotation,
+                                             float *dL_dopacity, void *stream);
+
 /* _C.get_local2j_ids_bool -- /root/reference/gaussian_renderer/workload_division.py:721-744.
  * strategy: (world_size+1) int32 ascending flattened tile ids; out: (P, world_size) uint8/bool. */
 GS_API int gs_get_local2j_ids_bool(int P, int image_height, int image_width, int world_size, const float *means2D,
@@ -419,6 +475,13 @@ GS_API int gs_sparse_grad_pack(int P, const uint8_t *mask, const int32_t *pos, v
                                void *stream);
 GS_API int gs_sparse_grad_unpack(int P, const uint8_t *mask, const int32_t *pos, const float *rows,
                                  void *const *grads_host, void *stream);
+/* The same for a model that stores rest_floats = 3 (K-1) floats of _features_rest per Gaussian (0, 9, 24 or 45 at
+ * max_sh_degree 0..3, gaussian_model.py:150-156): rows of 14 + rest_floats = 11 + 3 K floats, in the order above.  The rest
+ * gradient pointer may be NULL when rest_floats == 0.  gs_sparse_grad_pack / _unpack are these with rest_floats = 45. */
+GS_API int gs_sparse_grad_pack_rows(int P, int rest_floats, const uint8_t *mask, const int32_t *pos,
+                                    void *const *grads_host, float *rows, void *stream);
+GS_API int gs_sparse_grad_unpack_rows(int P, int rest_floats, const uint8_t *mask, const int32_t *pos,
+                                      const float *rows, void *const *grads_host, void *stream);
 
 /* ---- fused Adam step (SURVEY.md 8f rank 3) -- /root/reference/train_internal.py:316-329 ---------------------------
  * torch.optim.Adam(l, lr=0.0, eps=1e-15) over the six parameter groups (scene/gaussian_model.py:257-292), preceded by
