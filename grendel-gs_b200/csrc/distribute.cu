@@ -430,16 +430,12 @@ extern "C" int gs_xchg_scatter_grad(int B, int P, int W, const uint8_t *flags, c
     return GS_OK;
 }
 
-// ---- exchange over NVLink peer memory: pack + transfer in ONE kernel ---------------------------------------------
+// ---- NVLink peer memory for the direct-placement exchange below ---------------------------------------------------
 // all_to_all_single moves a rank's rows through NCCL's point-to-point channels: two device copies (pack into the send
 // buffer, NCCL from there into the peer's receive buffer) and a few channels per peer pair, far above the NVLink wire
-// time of the rows.  Here every rank's receive
-// buffer is a cudaMalloc allocation exported through CUDA IPC and mapped by all peers, and the pack kernel stores each
-// row straight into ITS FINAL ROW of the destination's buffer:
-//     row in rank j's buffer = recv_base_j[me] + (gpos - send_base_me[j])        (both bases follow from the counts)
-// A warp compacts the rows it owns for one destination in shared memory and writes them with coalesced 128-byte
-// stores, which is what NVLink wants.  The same kernel serves the local part (destination == me).  The backward is the
-// mirror image: gradient rows go straight into the row of the SOURCE rank's buffer its scatter kernel reads.
+// time of the rows.  Here every rank's receive region and gradient region are cudaMalloc allocations exported through
+// CUDA IPC and mapped by all peers: the pack kernel stores each splat straight into its final row of the destination's
+// receive region, and the backward loads the gradient rows straight from the destinations' gradient regions.
 // Ordering: the host enqueues a 4-byte all-reduce after the kernel; it completes on a rank once every peer's kernel has
 // finished, so the consumer that follows it in stream order sees all rows.  Buffers are reused every step: a peer only
 // writes after it has received this rank's counts of the NEXT step, which this rank sends after its consumers ran.
@@ -475,147 +471,6 @@ extern "C" int gs_peer_close(void *peer_ptr) {
 
 extern "C" int gs_peer_free(void *dev_ptr) {
     if (dev_ptr) GS_CUDA_TRY(cudaFree(dev_ptr));
-    return GS_OK;
-}
-
-// The active lanes of a warp each own one row of NF floats destined for `dst` (rows of lanes with consecutive active
-// ranks are adjacent in memory when they go to the same buffer): compact them in shared memory, then store
-// element-wise with consecutive lanes on consecutive addresses.
-template <int NF>
-GS_D void warp_store_rows(bool active, float *dst, const float (&v)[NF], float *s_val, float **s_ptr, int lane) {
-    const uint32_t mask = __ballot_sync(0xffffffffu, active);
-    if (mask == 0u) return;
-    const int q = __popc(mask & ((1u << lane) - 1u));
-    if (active) {
-#pragma unroll
-        for (int c = 0; c < NF; c++) s_val[q * NF + c] = v[c];
-        s_ptr[q] = dst;
-    }
-    __syncwarp();
-    const int n = __popc(mask) * NF;
-    for (int t = lane; t < n; t += 32) {
-        const int r = t / NF, c = t - r * NF;
-        s_ptr[r][c] = s_val[t];
-    }
-    __syncwarp();
-}
-
-struct XPeers { float *base[XW]; int32_t delta[XW]; };  // destination buffer of rank j and (its row) - (my send row)
-
-__global__ void __launch_bounds__(DT_THREADS)
-k_xchg_pack_p2p(int B, int P, int Wr, XIn in, const uint8_t *__restrict__ flags, const int32_t *__restrict__ gpos,
-                XPeers peers) {
-    __shared__ float s_val[DT_THREADS / 32][32 * ROW_FLOATS];
-    __shared__ float *s_ptr[DT_THREADS / 32][32];
-    const int i = blockIdx.x * DT_THREADS + threadIdx.x, k = blockIdx.y;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool valid = i < P;
-    bool any = false;
-    if (valid)
-        for (int j = 0; j < Wr; j++) any |= flags[((size_t)j * B + k) * P + i] != 0;
-    float v[ROW_FLOATS];
-#pragma unroll
-    for (int c = 0; c < ROW_FLOATS; c++) v[c] = 0.f;
-    if (any) {
-        const float2 m = *reinterpret_cast<const float2 *>(in.m2[k] + 2 * i);
-        const float4 co = *reinterpret_cast<const float4 *>(in.co[k] + 4 * i);
-        v[0] = m.x; v[1] = m.y;
-        v[2] = in.rgb[k][3 * i]; v[3] = in.rgb[k][3 * i + 1]; v[4] = in.rgb[k][3 * i + 2];
-        v[5] = co.x; v[6] = co.y; v[7] = co.z; v[8] = co.w;
-        v[9] = (float)in.rad[k][i]; v[10] = in.dep[k][i];
-    }
-    if (!__any_sync(0xffffffffu, any)) return;
-    for (int j = 0; j < Wr; j++) {
-        const size_t e = ((size_t)j * B + k) * P + (valid ? i : 0);
-        const bool hit = any && flags[e] != 0;
-        float *dst = hit ? peers.base[j] + ((size_t)gpos[e] + peers.delta[j]) * ROW_FLOATS : nullptr;
-        warp_store_rows<ROW_FLOATS>(hit, dst, v, s_val[warp], s_ptr[warp], lane);
-    }
-    __threadfence_system();
-}
-
-// dst_rows_ptrs_host[j]: rank j's receive buffer as mapped into this process (this rank's own buffer for j == me);
-// row_delta_host[j] = recv_base_j[me] - send_base_me[j].
-extern "C" int gs_xchg_pack_p2p(int B, int P, int W, const uint8_t *flags, const int32_t *gpos,
-                                const void *const *means2D_ptrs_host, const void *const *rgb_ptrs_host,
-                                const void *const *conic_opacity_ptrs_host, const void *const *radii_ptrs_host,
-                                const void *const *depths_ptrs_host, void *const *dst_rows_ptrs_host,
-                                const int32_t *row_delta_host, void *stream) {
-    GS_REQUIRE(B > 0 && B <= XB && W > 0 && W <= XW && P >= 0, "sizes");
-    if (P == 0) return GS_OK;
-    GS_REQUIRE(flags && gpos && means2D_ptrs_host && rgb_ptrs_host && conic_opacity_ptrs_host && radii_ptrs_host &&
-                   depths_ptrs_host && dst_rows_ptrs_host && row_delta_host, "null pointer");
-    XIn in;
-    fill_in(in, B, means2D_ptrs_host, rgb_ptrs_host, conic_opacity_ptrs_host, radii_ptrs_host, depths_ptrs_host);
-    XPeers peers;
-    for (int j = 0; j < XW; j++) {
-        peers.base[j] = j < W ? (float *)dst_rows_ptrs_host[j] : nullptr;
-        peers.delta[j] = j < W ? row_delta_host[j] : 0;
-        GS_REQUIRE(j >= W || peers.base[j] != nullptr, "null destination buffer");
-    }
-    GsStageTimer timer(GS_STAGE_PACK, (cudaStream_t)stream);
-    dim3 grid((P + DT_THREADS - 1) / DT_THREADS, B);
-    k_xchg_pack_p2p<<<grid, DT_THREADS, 0, (cudaStream_t)stream>>>(B, P, W, in, flags, gpos, peers);
-    GS_LAUNCH_CHECK();
-    return GS_OK;
-}
-
-struct XSegPeers { float *base[XSEG]; };  // per recv segment: first gradient row of that block in the SOURCE's buffer
-
-__global__ void __launch_bounds__(DT_THREADS)
-k_xchg_pack_grad_p2p(int total, XSegs segs, XIn g, XSegPeers dst) {
-    __shared__ float s_val[DT_THREADS / 32][32 * GRAD_FLOATS];
-    __shared__ float *s_ptr[DT_THREADS / 32][32];
-    const int r = blockIdx.x * DT_THREADS + threadIdx.x;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool valid = r < total;
-    float v[GRAD_FLOATS];
-#pragma unroll
-    for (int t = 0; t < GRAD_FLOATS; t++) v[t] = 0.f;
-    float *out = nullptr;
-    if (valid) {
-        const int s = xseg_find(segs, r);
-        const int k = segs.cam[s], off = r - segs.recv_start[s], i = segs.dst_start[s] + off;
-        if (g.m2[k]) { v[0] = g.m2[k][2 * i]; v[1] = g.m2[k][2 * i + 1]; }
-        if (g.rgb[k]) { v[2] = g.rgb[k][3 * i]; v[3] = g.rgb[k][3 * i + 1]; v[4] = g.rgb[k][3 * i + 2]; }
-        if (g.co[k]) {
-            const float4 c = *reinterpret_cast<const float4 *>(g.co[k] + 4 * i);
-            v[5] = c.x; v[6] = c.y; v[7] = c.z; v[8] = c.w;
-        }
-        out = dst.base[s] + (size_t)off * GRAD_FLOATS;
-    }
-    warp_store_rows<GRAD_FLOATS>(valid, out, v, s_val[warp], s_ptr[warp], lane);
-    __threadfence_system();
-}
-
-// seg_dst_ptrs_host[q]: address (in this process) of the FIRST gradient row of segment q inside the source rank's
-// gradient buffer, i.e. base_of_rank_i + (row where rank i packed its (camera k -> me) block) * 9 floats.  Segments as
-// in gs_xchg_unpack; only the non-empty ones are used.
-extern "C" int gs_xchg_pack_grad_p2p(int nseg, const int32_t *seg_recv_start_host, const int32_t *seg_len_host,
-                                     const int32_t *seg_cam_host, const int32_t *seg_dst_start_host, int total_rows,
-                                     int B, const void *const *d_means2D_ptrs_host, const void *const *d_rgb_ptrs_host,
-                                     const void *const *d_conic_opacity_ptrs_host, void *const *seg_dst_ptrs_host,
-                                     void *stream) {
-    GS_REQUIRE(B > 0 && B <= XB && total_rows >= 0, "sizes");
-    if (total_rows == 0) return GS_OK;
-    GS_REQUIRE(seg_dst_ptrs_host && d_means2D_ptrs_host && d_rgb_ptrs_host && d_conic_opacity_ptrs_host, "null pointer");
-    XSegs s;
-    int rc = fill_segs(s, nseg, seg_recv_start_host, seg_len_host, seg_cam_host, seg_dst_start_host);
-    if (rc != GS_OK) return rc;
-    XSegPeers dst;
-    int n = 0;  // same compaction as fill_segs: empty segments are dropped
-    for (int q = 0; q < nseg; q++) {
-        if (seg_len_host[q] <= 0) continue;
-        GS_REQUIRE(seg_dst_ptrs_host[q] != nullptr, "null destination buffer");
-        dst.base[n++] = (float *)seg_dst_ptrs_host[q];
-    }
-    for (int q = n; q < XSEG; q++) dst.base[q] = nullptr;
-    XIn g;
-    fill_in(g, B, d_means2D_ptrs_host, d_rgb_ptrs_host, d_conic_opacity_ptrs_host, nullptr, nullptr);
-    GsStageTimer timer(GS_STAGE_UNPACK, (cudaStream_t)stream);
-    k_xchg_pack_grad_p2p<<<(total_rows + DT_THREADS - 1) / DT_THREADS, DT_THREADS, 0, (cudaStream_t)stream>>>(total_rows,
-                                                                                                              s, g, dst);
-    GS_LAUNCH_CHECK();
     return GS_OK;
 }
 
@@ -708,10 +563,10 @@ extern "C" int gs_sparse_grad_unpack(int P, const uint8_t *mask, const int32_t *
     return gs_sparse_grad_unpack_rows(P, 45, mask, pos, rows, grads_host, stream);
 }
 
-// ---- direct-placement exchange (round 2) ---------------------------------------------------------------------------
-// The first peer-memory exchange still materialised a dense [destination][camera][splat] flag array, a W*B*P-element
-// scan (64 MB of positions at W = B = 8), a row-major staging layout and an unpack pass on the receiver, all of it
-// traffic the rows themselves do not need.  Here:
+// ---- direct-placement exchange ---------------------------------------------------------------------------------------
+// The row-staged exchange above materialises a dense [destination][camera][splat] flag array, a W*B*P-element scan
+// (64 MB of positions at W = B = 8), a row-major staging layout and an unpack pass on the receiver, all of it traffic
+// the rows themselves do not need.  Here:
 //   * routing is recomputed from (means2D, radius) wherever it is needed (12 B per splat) instead of being stored;
 //   * positions come from per-CTA hit counts ([destination][camera][block of 256 splats]: W*B*P/256 integers, scanned
 //     in microseconds) plus a ballot prefix inside the CTA -- the order is still the reference's (per destination:
@@ -813,7 +668,7 @@ __global__ void __launch_bounds__(DT_THREADS)
 k_xr_pack(XrGeom g, XIn in, const int32_t *__restrict__ blkbase, XrPeers peers, const int32_t *__restrict__ row0_dev) {
     __shared__ int32_t s_wcnt[DT_THREADS / 32][XW];
     __shared__ float s_rgb[DT_THREADS / 32][96];
-    if (row0_dev != nullptr && row0_dev[g.Wr * g.B] != 0) return;   // over capacity: nothing is written (uniform)
+    if (row0_dev[g.Wr * g.B] != 0) return;   // over capacity: nothing is written (uniform)
     const int i = blockIdx.x * DT_THREADS + threadIdx.x, k = blockIdx.y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const bool valid = i < g.P;
@@ -849,8 +704,7 @@ k_xr_pack(XrGeom g, XIn in, const int32_t *__restrict__ blkbase, XrPeers peers, 
         for (int w = 0; w < warp; w++) lr += s_wcnt[w][j];
         const bool hit = (h >> j) & 1u;
         const size_t col = (size_t)j * g.B + k;
-        const long long row = (long long)(row0_dev ? row0_dev[col] : peers.row0[col]) +
-                              (blkbase[col * gridDim.x + blockIdx.x] - blkbase[col * gridDim.x]) + lr;
+        const long long row = (long long)row0_dev[col] + (blkbase[col * gridDim.x + blockIdx.x] - blkbase[col * gridDim.x]) + lr;
         float *b = reinterpret_cast<float *>(peers.base[j]);
         if (hit) {
             *reinterpret_cast<float2 *>(b + 2 * row) = m;
@@ -864,79 +718,6 @@ k_xr_pack(XrGeom g, XIn in, const int32_t *__restrict__ blkbase, XrPeers peers, 
         float *q = b + 2 * cap + 3 * row_w;
         for (int t = lane; t < 3 * wn; t += 32) q[t] = s_rgb[warp][t];
         __syncwarp();
-    }
-}
-
-// CTA-level compaction (round 2, last step): k_xr_pack lets every WARP store its own hits, and at 8 ranks a warp has ~4
-// hits per destination -- 32-byte means2D spans, 48-byte rgb spans: NVLink write packets far below a cache line.  Here the
-// CTA's hits for one destination (consecutive rows, in thread order: the same rows as k_xr_pack) are staged in shared
-// memory and written by consecutive threads, one row per thread: ~27 rows = 216 / 432 / 324-byte spans per field.
-__global__ void __launch_bounds__(DT_THREADS)
-k_xr_pack_cta(XrGeom g, XIn in, const int32_t *__restrict__ blkbase, XrPeers peers, const int32_t *__restrict__ row0_dev) {
-    __shared__ int32_t s_wcnt[DT_THREADS / 32][XW];
-    __shared__ float2 s_m2[DT_THREADS];
-    __shared__ float4 s_co[DT_THREADS];
-    __shared__ float s_rgb[3 * DT_THREADS];
-    __shared__ int32_t s_rad[DT_THREADS];
-    __shared__ float s_dep[DT_THREADS];
-    __shared__ uint32_t s_any[DT_THREADS / 32];
-    if (row0_dev != nullptr && row0_dev[g.Wr * g.B] != 0) return;   // over capacity: nothing is written (uniform)
-    const int i = blockIdx.x * DT_THREADS + threadIdx.x, k = blockIdx.y;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool valid = i < g.P;
-    const uint32_t h = xr_hits(g, k, i, valid);
-    const uint32_t wany = __reduce_or_sync(0xffffffffu, h);
-    for (int j = 0; j < g.Wr; j++) {
-        const int c = __popc(__ballot_sync(0xffffffffu, (h >> j) & 1u));
-        if (lane == 0) s_wcnt[warp][j] = c;
-    }
-    if (lane == 0) s_any[warp] = wany;
-    __syncthreads();
-    uint32_t any = 0u;
-#pragma unroll
-    for (int w = 0; w < DT_THREADS / 32; w++) any |= s_any[w];
-    if (any == 0u) return;
-    float2 m = make_float2(0.f, 0.f);
-    float4 co = make_float4(0.f, 0.f, 0.f, 0.f);
-    float r0 = 0.f, r1 = 0.f, r2 = 0.f, dep = 0.f;
-    int rad = 0;
-    if (h) {
-        m = *reinterpret_cast<const float2 *>(in.m2[k] + 2 * (size_t)i);
-        co = *reinterpret_cast<const float4 *>(in.co[k] + 4 * (size_t)i);
-        r0 = in.rgb[k][3 * (size_t)i]; r1 = in.rgb[k][3 * (size_t)i + 1]; r2 = in.rgb[k][3 * (size_t)i + 2];
-        rad = in.rad[k][i]; dep = in.dep[k][i];
-    }
-    const long long cap = peers.cap;
-    while (any) {
-        const int j = __ffs(any) - 1;
-        any &= any - 1u;
-        const uint32_t bal = __ballot_sync(0xffffffffu, (h >> j) & 1u);
-        int lr = __popc(bal & ((1u << lane) - 1u)), cnt = 0;
-#pragma unroll
-        for (int w = 0; w < DT_THREADS / 32; w++) {
-            const int c = s_wcnt[w][j];
-            if (w < warp) lr += c;
-            cnt += c;
-        }
-        if ((h >> j) & 1u) {   // rank lr among the CTA's hits for destination j = its row offset
-            s_m2[lr] = m; s_co[lr] = co; s_rad[lr] = rad; s_dep[lr] = dep;
-            s_rgb[3 * lr] = r0; s_rgb[3 * lr + 1] = r1; s_rgb[3 * lr + 2] = r2;
-        }
-        __syncthreads();
-        const size_t col = (size_t)j * g.B + k;
-        const long long row = (long long)(row0_dev ? row0_dev[col] : peers.row0[col]) +
-                              (blkbase[col * gridDim.x + blockIdx.x] - blkbase[col * gridDim.x]);   // the CTA's first row
-        float *b = reinterpret_cast<float *>(peers.base[j]);
-        const int t = threadIdx.x;
-        if (t < cnt) {
-            reinterpret_cast<float2 *>(b + 2 * row)[t] = s_m2[t];
-            reinterpret_cast<float4 *>(b + 5 * cap + 4 * row)[t] = s_co[t];
-            reinterpret_cast<int32_t *>(b + 9 * cap)[row + t] = s_rad[t];
-            (b + 10 * cap)[row + t] = s_dep[t];
-        }
-        float *q = b + 2 * cap + 3 * row;
-        for (int u = t; u < 3 * cnt; u += DT_THREADS) q[u] = s_rgb[u];
-        __syncthreads();   // the staging arrays are reused for the next destination
     }
 }
 
@@ -1040,35 +821,11 @@ extern "C" int gs_xr_count(int B, int P, int W, int image_height, int image_widt
 }
 
 // peer_recv_ptrs_host[j]: rank j's receive region (11 * cap floats: means2D | rgb | conic_opacity | radii | depths) as
-// mapped into this process; dst_row0_host[j*B+k]: first row of THIS rank's block inside camera k of rank j's arrays.
-extern "C" int gs_xr_pack(int B, int P, int W, int image_height, int image_width, const void *const *means2D_ptrs_host,
-                          const void *const *rgb_ptrs_host, const void *const *conic_opacity_ptrs_host,
-                          const void *const *radii_ptrs_host, const void *const *depths_ptrs_host,
-                          const int32_t *row_lo_host, const int32_t *row_hi_host, const int32_t *blkbase,
-                          void *const *peer_recv_ptrs_host, const int32_t *dst_row0_host, long long cap_rows, void *stream) {
-    XrGeom g;
-    int rc = xr_geom(g, B, P, W, image_height, image_width, means2D_ptrs_host, radii_ptrs_host, row_lo_host, row_hi_host);
-    if (rc != GS_OK) return rc;
-    if (P == 0) return GS_OK;
-    GS_REQUIRE(rgb_ptrs_host && conic_opacity_ptrs_host && depths_ptrs_host && blkbase, "null pointer");
-    XrPeers peers;
-    rc = xr_peers(peers, B, W, peer_recv_ptrs_host, dst_row0_host, cap_rows);
-    if (rc != GS_OK) return rc;
-    XIn in;
-    fill_in(in, B, means2D_ptrs_host, rgb_ptrs_host, conic_opacity_ptrs_host, radii_ptrs_host, depths_ptrs_host);
-    GsStageTimer timer(GS_STAGE_PACK, (cudaStream_t)stream);
-    if (g_gs_debug_flags & GS_DEBUG_XR_PACK_CTA)
-        k_xr_pack_cta<<<dim3(XR_NB(P), B), DT_THREADS, 0, (cudaStream_t)stream>>>(g, in, blkbase, peers, nullptr);
-    else
-        k_xr_pack<<<dim3(XR_NB(P), B), DT_THREADS, 0, (cudaStream_t)stream>>>(g, in, blkbase, peers, nullptr);
-    GS_LAUNCH_CHECK();
-    return GS_OK;
-}
-
-// gs_xr_pack with the destination rows computed on the device: counts_all_dev = the all-gathered counts (W*B*W int32,
-// [source i][camera k][destination j], as all_gather_into_tensor of every rank's (B,W) table leaves them), me = this rank,
-// row0_dev = (W*B + 1) int32 scratch that receives the rows and the over-capacity flag.  The caller needs no host copy of
-// the counts to launch it: the launch goes out right behind the all-gather and the host reads the counts while it runs.
+// mapped into this process.  The destination rows are computed on the device: counts_all_dev = the all-gathered counts
+// (W*B*W int32, [source i][camera k][destination j], as all_gather_into_tensor of every rank's (B,W) table leaves them),
+// me = this rank, row0_dev = (W*B + 1) int32 scratch that receives the rows and the over-capacity flag.  The caller needs
+// no host copy of the counts to launch it: the launch goes out right behind the all-gather and the host reads the
+// counts while it runs.
 extern "C" int gs_xr_pack_dev(int B, int P, int W, int image_height, int image_width, const void *const *means2D_ptrs_host,
                               const void *const *rgb_ptrs_host, const void *const *conic_opacity_ptrs_host,
                               const void *const *radii_ptrs_host, const void *const *depths_ptrs_host,
@@ -1081,7 +838,7 @@ extern "C" int gs_xr_pack_dev(int B, int P, int W, int image_height, int image_w
     GS_REQUIRE(counts_all_dev && row0_dev && me >= 0 && me < W, "device counts / row table / rank");
     GS_REQUIRE(W * B <= 256, "W * B <= 256");
     XrPeers peers;
-    int32_t zeros[XW * XB] = {0};
+    int32_t zeros[XW * XB] = {0};   // k_xr_pack reads its rows from row0_dev
     rc = xr_peers(peers, B, W, peer_recv_ptrs_host, zeros, cap_rows);
     if (rc != GS_OK) return rc;
     k_xr_rows<<<1, 256, 0, (cudaStream_t)stream>>>(W, B, me, counts_all_dev, cap_rows, row0_dev);
@@ -1091,10 +848,7 @@ extern "C" int gs_xr_pack_dev(int B, int P, int W, int image_height, int image_w
     XIn in;
     fill_in(in, B, means2D_ptrs_host, rgb_ptrs_host, conic_opacity_ptrs_host, radii_ptrs_host, depths_ptrs_host);
     GsStageTimer timer(GS_STAGE_PACK, (cudaStream_t)stream);
-    if (g_gs_debug_flags & GS_DEBUG_XR_PACK_CTA)
-        k_xr_pack_cta<<<dim3(XR_NB(P), B), DT_THREADS, 0, (cudaStream_t)stream>>>(g, in, blkbase, peers, row0_dev);
-    else
-        k_xr_pack<<<dim3(XR_NB(P), B), DT_THREADS, 0, (cudaStream_t)stream>>>(g, in, blkbase, peers, row0_dev);
+    k_xr_pack<<<dim3(XR_NB(P), B), DT_THREADS, 0, (cudaStream_t)stream>>>(g, in, blkbase, peers, row0_dev);
     GS_LAUNCH_CHECK();
     return GS_OK;
 }

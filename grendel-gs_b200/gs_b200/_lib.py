@@ -98,11 +98,8 @@ SIGNATURES = {
     "gs_peer_open": (_i, [_vp, C.POINTER(C.c_void_p)]),
     "gs_peer_close": (_i, [_vp]),
     "gs_peer_free": (_i, [_vp]),
-    "gs_xchg_pack_p2p": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "gs_xchg_pack_grad_p2p": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "gs_xr_temp_bytes": (_sz, [_i, _i, _i]),
     "gs_xr_count": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "gs_xr_pack": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_longlong, _vp]),
     "gs_xr_pack_dev": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, C.c_longlong, _vp]),
     "gs_xr_pull_grad": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_longlong, _vp, _vp, _vp, _vp]),
     "gs_sparse_grad_mask": (_i, [_i, _vp, _vp, _vp]),
@@ -163,7 +160,6 @@ STAGE_NUM = 14
 DEBUG_NO_BLOCK_CULL = 1
 DEBUG_BWD_TILE = 2       # gs_render_backward: round 1's tile-parallel kernel instead of the segment-parallel one
 DEBUG_FWD_HALFWARP = 4   # gs_render_forward: round 1's half-warp blend kernel instead of the packed two-pixel one
-DEBUG_XR_PACK_CTA = 8    # direct exchange: CTA-compacted pack kernel (A/B switch)
 
 
 def debug_set(flags):

@@ -2,15 +2,17 @@
 
 Restates /root/reference/gaussian_renderer/__init__.py:542-698 (all_to_all_communication_final):
 every rank projects its own Gaussian shard for all B cameras, then sends each projected splat to the
-ranks whose tile-row strip its rectangle touches.  Differences from the reference's Python glue:
-  * ONE launch per stage for all B cameras: routing flags are laid out [destination][camera][splat], so a single
-    exclusive scan yields every row of the send buffer and the pack kernel writes straight into it (no W x B
-    nonzero()/index_select/cat, workload_division.py:741-742, __init__.py:590-607);
-  * ONE all_to_all_single of 11-float rows forward (means2D, rgb, conic_opacity, radius, depth) instead
-    of two collectives, ONE of 9-float rows backward; one host sync (the counts) instead of W+2;
-  * the backward scatter is one thread per local splat (no atomics).
-Row order is the reference's: per destination, cameras in batch order, splats in index order; per
-receiver, sources in rank order.
+ranks whose tile-row strip its rectangle touches.  Two paths, chosen per step from values every rank shares:
+  * direct placement over NVLink peer memory (PeerBuffers, default when every rank could map them): the pack kernel
+    stores every splat into its final row of the destination's receive region, which IS the render's input, and the
+    backward pulls the gradient rows from the destinations' gradient regions;
+  * row staging over NCCL (no peer buffers, or a step whose rows exceed them): ONE launch per stage for all B cameras
+    -- routing flags are laid out [destination][camera][splat], so a single exclusive scan yields every row of the
+    send buffer (no W x B nonzero()/index_select/cat, workload_division.py:741-742, __init__.py:590-607) -- ONE
+    all_to_all_single of 11-float rows forward (means2D, rgb, conic_opacity, radius, depth) instead of two
+    collectives, ONE of 9-float rows backward, and a backward scatter of one thread per local splat (no atomics).
+Both need one host sync (the counts) instead of W+2.  Row order is the reference's: per destination, cameras in batch
+order, splats in index order; per receiver, sources in rank order.
 """
 import ctypes as C
 
@@ -22,13 +24,7 @@ from . import _lib, ops
 
 ROW, GROW = 11, 9
 MAX_CAMERAS, MAX_RANKS, MAX_SEGMENTS = 16, 16, 128   # XB, XW, XSEG of csrc/distribute.cu
-# "direct": direct-placement kernels over peer memory (default when peer buffers exist); "rows": round 1's row-staged
-# peer path (pack rows -> unpack), kept for A/B (GS_B200_EXCHANGE_MODE=rows)
-import os as _os
-MODE = _os.environ.get("GS_B200_EXCHANGE_MODE", "direct")
-# destination rows of the direct pack computed on the device, counts read on a side stream (no dry main stream at the
-# exchange's host sync); GS_B200_XR_DEVROWS=0: the host computes the rows before the pack is launched
-DEVICE_ROWS = _os.environ.get("GS_B200_XR_DEVROWS", "1") == "1"
+MODE = "direct"   # the exchange over peer memory: direct placement (bench.py reports it)
 TRACE = None   # diagnostics: callable(name) that synchronises and charges the time since the last mark (pipeline._mark)
 
 
@@ -166,10 +162,11 @@ def _slab_ptrs(t, B):
 
 
 class PeerBuffers:
-    """NVLink peer-memory exchange buffers (include/grendel_gs_b200.h, gs_peer_* / gs_xchg_*_p2p): every rank owns one
-    receive buffer of `cap_rows` 11-float rows and one gradient buffer of `cap_rows` 9-float rows, exported over CUDA
-    IPC and mapped by all peers of the node.  recv[j] / grad[j] are rank j's buffers as addresses valid in THIS process.
-    Collective: every rank of `group` must construct it at the same point (handles travel by all_gather)."""
+    """NVLink peer-memory regions of the direct-placement exchange (include/grendel_gs_b200.h, gs_peer_* / gs_xr_*):
+    every rank owns one receive region of `cap_rows` rows (means2D | rgb | conic_opacity | radii | depths, 11 floats per
+    row) and one gradient region of `cap_rows` rows (d means2D | d rgb | d conic_opacity, 10 floats per row), exported
+    over CUDA IPC and mapped by all peers of the node.  recv[j] / grad[j] are rank j's regions as addresses valid in THIS
+    process.  Collective: every rank of `group` must construct it at the same point (handles travel by all_gather)."""
 
     def __init__(self, world, me, cap_rows, device, group=None):
         self.world, self.me, self.cap_rows, self.group = world, me, (int(cap_rows) + 3) // 4 * 4, group
@@ -181,8 +178,7 @@ class PeerBuffers:
         # or all ranks raise -- never a rank stuck alone in a collective
         handles, err = [0] * 128, None
         try:
-            # gradient buffer: 10 floats per row (the direct-placement layout pads d rgb to 16 bytes; the row-staged path
-            # uses 9 of them)
+            # gradient region: 10 floats per row (d rgb is padded to 16 bytes)
             for q, nbytes in enumerate((self.cap_rows * ROW * 4, self.cap_rows * (GROW + 1) * 4)):
                 ptr, handle = C.c_void_p(), (C.c_ubyte * 64)()
                 _lib.call("gs_peer_alloc", nbytes, C.byref(ptr), handle)
@@ -221,12 +217,14 @@ class PeerBuffers:
         """Stream-ordered: completes on this rank once every rank's stream reached the same call (a 4-byte all-reduce;
         the host does not block).
 
-        Buffer-reuse invariant (ADVICE r1): a peer writes into this rank's recv / grad buffer only from its pack kernels,
-        and it launches those only after gather_counts() of the SAME exchange -- an all-gather on the same stream that
-        this rank joins after its unpack / scatter of the previous exchange were enqueued.  So the next remote write is
-        ordered after this rank's last read as long as (a) every exchange starts with gather_counts and (b) exchange,
-        consumers and collectives share one stream.  A caller that caches counts or moves the consumers to another stream
-        must call barrier() after its consumers instead."""
+        Buffer-reuse invariant: a peer writes into this rank's receive region only from its pack kernel, and it launches
+        that only after the all-gather of the SAME exchange's counts; it reads this rank's gradient region only in its
+        pull kernel, which it enqueues before it joins the next exchange's all-gather.  Those all-gathers run on the
+        stream that this rank joins after its consumers of the previous exchange (the render reading the receive region,
+        the backward writing the gradient region) were enqueued.  So every remote access is ordered against this rank's
+        own accesses as long as (a) every exchange starts with the all-gather of the counts and (b) exchange, consumers
+        and collectives share one stream.  A caller that caches counts or moves the consumers to another stream must call
+        barrier() after its consumers instead."""
         dist.all_reduce(self.token, op=dist.ReduceOp.MAX, group=self.group)   # MAX of zeros: the value never grows
 
     def views(self):
@@ -245,11 +243,6 @@ class PeerBuffers:
     def fits_direct(self, cnt):
         """Do every rank's received rows (all cameras) fit the structure-of-arrays regions?  Same answer on every rank."""
         return int(np.asarray(cnt, dtype=np.int64).sum(axis=(0, 1)).max()) <= self.cap_rows
-
-    def fits(self, cnt):
-        """Do all ranks' receive and send totals of this step fit the buffers?  Same answer on every rank."""
-        S = np.asarray(cnt, dtype=np.int64).sum(axis=1)     # S[i][j]: rows i -> j
-        return int(max(S.sum(axis=0).max(), S.sum(axis=1).max())) <= self.cap_rows
 
     def close(self):
         for name, ptrs in (("gs_peer_close", self._opened), ("gs_peer_free", self._owned)):
@@ -285,22 +278,6 @@ def direct_rows(cnt, me):
     return row0.reshape(-1).tolist(), [int(v) for v in mine]
 
 
-def peer_row_deltas(cnt, me):
-    """delta[j] = (first row of my block in rank j's receive buffer) - (first row of my block for j in my send order):
-    a row packed at position gpos of the send order lands in row gpos + delta[j] of rank j's buffer."""
-    S = np.asarray(cnt, dtype=np.int64).sum(axis=1)         # S[i][j]: rows i -> j
-    recv_base = S[:me].sum(axis=0)                          # [j]: rows of ranks < me in rank j's buffer
-    return (recv_base - _excl(S[me])).tolist()
-
-
-def peer_grad_rows(cnt, me):
-    """For every (source rank i, camera k) segment of my receive buffer, in segments() order: the row of rank i's SEND
-    order where its (camera k -> me) block starts -- where my gradient rows for that block have to go."""
-    c = np.asarray(cnt, dtype=np.int64)
-    base = c[:, :, :me].sum(axis=(1, 2))                    # [i]: rows rank i sends to ranks < me
-    return (base[:, None] + _excl(c[:, :, me], axis=1)).reshape(-1).tolist()
-
-
 def _row_ptrs(t, starts, B):
     """Device pointers of rows starts[k] (k < B) of a contiguous (N, ...) tensor; NULLs if t is None."""
     if t is None:
@@ -326,24 +303,13 @@ class _ExchangeSplats(torch.autograd.Function):
         radii, depths = state["radii"], state["depths"]
         dev = m2.device
         s = ops._stream()
-        peer = state["peer"]
-        if peer is not None:
-            # pack + transfer in one kernel: rows go straight into their final rows of the destinations' buffers
-            _lib.call("gs_xchg_pack_p2p", B, P, W, state["flags"].data_ptr(), state["gpos"].data_ptr(), _slab_ptrs(m2, B),
-                      _slab_ptrs(rgb, B), _slab_ptrs(co, B), _slab_ptrs(radii, B), _slab_ptrs(depths, B),
-                      (C.c_void_p * W)(*peer.recv), _i32(peer_row_deltas(state["cnt"], state["me"])), s)
-            _t("x3 pack")
-            peer.barrier()
-            recv_ptr = peer.recv[state["me"]]
-        else:
-            send = torch.empty((max(layout.total_send, 1), ROW), dtype=torch.float32, device=dev)
-            _lib.call("gs_xchg_pack", B, P, W, state["flags"].data_ptr(), state["gpos"].data_ptr(), _slab_ptrs(m2, B),
-                      _slab_ptrs(rgb, B), _slab_ptrs(co, B), _slab_ptrs(radii, B), _slab_ptrs(depths, B), send.data_ptr(), s)
-            _t("x3 pack")
-            recv = torch.empty((max(layout.total_recv, 1), ROW), dtype=torch.float32, device=dev)
-            all_to_all_single(recv[:layout.total_recv], send[:layout.total_send], layout.recv_splits, layout.send_splits,
-                              group)
-            recv_ptr = recv.data_ptr()
+        send = torch.empty((max(layout.total_send, 1), ROW), dtype=torch.float32, device=dev)
+        _lib.call("gs_xchg_pack", B, P, W, state["flags"].data_ptr(), state["gpos"].data_ptr(), _slab_ptrs(m2, B),
+                  _slab_ptrs(rgb, B), _slab_ptrs(co, B), _slab_ptrs(radii, B), _slab_ptrs(depths, B), send.data_ptr(), s)
+        _t("x3 pack")
+        recv = torch.empty((max(layout.total_recv, 1), ROW), dtype=torch.float32, device=dev)
+        all_to_all_single(recv[:layout.total_recv], send[:layout.total_send], layout.recv_splits, layout.send_splits,
+                          group)
         _t("x4 all_to_all")
         vs = state["view_start"]
         N = vs[B]
@@ -353,7 +319,7 @@ class _ExchangeSplats(torch.autograd.Function):
         orad = torch.empty((N,), dtype=torch.int32, device=dev)
         odep = torch.empty((N,), dtype=torch.float32, device=dev)
         rs, ln, cam, ds = state["segs"]
-        _lib.call("gs_xchg_unpack", len(rs), _i32(rs), _i32(ln), _i32(cam), _i32(ds), layout.total_recv, recv_ptr,
+        _lib.call("gs_xchg_unpack", len(rs), _i32(rs), _i32(ln), _i32(cam), _i32(ds), layout.total_recv, recv.data_ptr(),
                   B, _row_ptrs(om2, vs, B), _row_ptrs(orgb, vs, B), _row_ptrs(oco, vs, B), _row_ptrs(orad, vs, B),
                   _row_ptrs(odep, vs, B), s)
         ctx.state = state
@@ -371,30 +337,18 @@ class _ExchangeSplats(torch.autograd.Function):
         _t("b1 loss+render backward")
         g_m2, g_rgb, g_co = (None if t is None else t.contiguous() for t in (g_m2, g_rgb, g_co))
         rs, ln, cam, ds = state["segs"]
-        peer = state["peer"]
-        if peer is not None:
-            # gradient rows go straight into the rows of the SOURCE ranks' buffers that their scatter kernels read
-            rows = peer_grad_rows(state["cnt"], state["me"])
-            dst = (C.c_void_p * len(rs))(*[peer.grad[q // B] + rows[q] * GROW * 4 for q in range(len(rs))])
-            _lib.call("gs_xchg_pack_grad_p2p", len(rs), _i32(rs), _i32(ln), _i32(cam), _i32(ds), layout.total_recv, B,
-                      _row_ptrs(g_m2, vs, B), _row_ptrs(g_rgb, vs, B), _row_ptrs(g_co, vs, B), dst, s)
-            _t("b2 pack_grad")
-            peer.barrier()
-            gsend_ptr = peer.grad[state["me"]]
-        else:
-            grecv = torch.empty((max(layout.total_recv, 1), GROW), dtype=torch.float32, device=dev)
-            _lib.call("gs_xchg_pack_grad", len(rs), _i32(rs), _i32(ln), _i32(cam), _i32(ds), layout.total_recv, B,
-                      _row_ptrs(g_m2, vs, B), _row_ptrs(g_rgb, vs, B), _row_ptrs(g_co, vs, B), grecv.data_ptr(), s)
-            _t("b2 pack_grad")
-            gsend = torch.empty((max(layout.total_send, 1), GROW), dtype=torch.float32, device=dev)
-            all_to_all_single(gsend[:layout.total_send], grecv[:layout.total_recv], layout.send_splits, layout.recv_splits,
-                              group)
-            gsend_ptr = gsend.data_ptr()
+        grecv = torch.empty((max(layout.total_recv, 1), GROW), dtype=torch.float32, device=dev)
+        _lib.call("gs_xchg_pack_grad", len(rs), _i32(rs), _i32(ln), _i32(cam), _i32(ds), layout.total_recv, B,
+                  _row_ptrs(g_m2, vs, B), _row_ptrs(g_rgb, vs, B), _row_ptrs(g_co, vs, B), grecv.data_ptr(), s)
+        _t("b2 pack_grad")
+        gsend = torch.empty((max(layout.total_send, 1), GROW), dtype=torch.float32, device=dev)
+        all_to_all_single(gsend[:layout.total_send], grecv[:layout.total_recv], layout.send_splits, layout.recv_splits,
+                          group)
         _t("b3 all_to_all")
         d_m2 = torch.empty((B, P, 2), dtype=torch.float32, device=dev)
         d_rgb = torch.empty((B, P, 3), dtype=torch.float32, device=dev)
         d_co = torch.empty((B, P, 4), dtype=torch.float32, device=dev)
-        _lib.call("gs_xchg_scatter_grad", B, P, W, state["flags"].data_ptr(), state["gpos"].data_ptr(), gsend_ptr,
+        _lib.call("gs_xchg_scatter_grad", B, P, W, state["flags"].data_ptr(), state["gpos"].data_ptr(), gsend.data_ptr(),
                   _slab_ptrs(d_m2, B), _slab_ptrs(d_rgb, B), _slab_ptrs(d_co, B), s)
         return None, d_m2, d_rgb, d_co
 
@@ -493,8 +447,8 @@ def exchange(means2D, rgb, conic_opacity, radii, depths, strategies, settings, w
 def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, settings, world, me, group=None, peer=None):
     """means2D (B,P,2), rgb (B,P,3), conic_opacity (B,P,4), radii (B,P) int32, depths (B,P): the local shard projected
     into the B cameras of the step (ops.preprocess_gaussians_batched, or torch.stack of per-camera results).
-    peer: PeerBuffers -> rows travel by direct NVLink stores from the pack kernels (steps whose totals exceed the
-    buffers, and peer=None, go through all_to_all_single).
+    peer: PeerBuffers -> splats travel by direct NVLink stores from the pack kernel into their final rows (steps where
+    some rank would receive more than the regions hold, and peer=None, go through all_to_all_single).
     Returns ((means2D (N,2), rgb (N,3), conic_opacity (N,4), radii (N), depths (N)), view_start, cnt): the splats this
     rank has to render, all cameras concatenated in camera order (camera k = rows [view_start[k], view_start[k+1]),
     none if the rank renders no strip of it), and the all-gathered counts cnt[i][k][j] (the reference's
@@ -514,7 +468,7 @@ def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, setting
     radii = radii.to(torch.int32).contiguous()
     depths = depths.contiguous()
     m2d = means2D.detach().contiguous()
-    if peer is not None and MODE == "direct":
+    if peer is not None:
         # direct placement: per-block hit counts instead of a dense flag array + W*B*P-element scan
         nblk = max(world * B * ((max(P, 1) + 255) // 256), 1)
         blkcnt = torch.empty((nblk,), dtype=torch.int32, device=dev)
@@ -526,8 +480,7 @@ def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, setting
         _lib.call("gs_xr_count", B, P, world, H, Wimg, _slab_ptrs(m2d, B), _slab_ptrs(radii, B), lo_c, hi_c,
                   blkcnt.data_ptr(), blkbase.data_ptr(), counts.data_ptr(), temp.data_ptr(), tb, ops._stream())
         _t("x1 route")
-        # everything the pack launch needs is prepared BEFORE the host waits for the counts: the GPU is idle from the
-        # all-gather until the pack kernel starts
+        # everything the pack launch needs is prepared BEFORE the all-gather is enqueued: the launch follows it closely
         rgb_c, co_c = rgb.detach().contiguous(), conic_opacity.detach().contiguous()
         pack_args = (B, P, world, H, Wimg, _slab_ptrs(m2d, B), _slab_ptrs(rgb_c, B), _slab_ptrs(co_c, B),
                      _slab_ptrs(radii, B), _slab_ptrs(depths, B), lo_c, hi_c, blkbase.data_ptr(),
@@ -537,36 +490,26 @@ def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, setting
         # (k_xr_rows), so pack + barrier are enqueued before the host knows the counts; the host copy of the counts -- needed
         # for the tensor shapes of the render -- is read on a side stream meanwhile.  The main stream does not run dry at the
         # exchange's host sync (the reference blocks on the sizes before its all-to-all, gaussian_renderer/__init__.py:609-628).
-        if DEVICE_ROWS:
-            flat = counts.t().contiguous().reshape(-1)                    # [camera k][destination j]
-            allc = torch.empty((world * flat.numel(),), dtype=torch.int32, device=dev)
-            dist.all_gather_into_tensor(allc, flat, group=group)          # cnt[i][k][j]
-            allp = _piggyback_gather(dev, world, group)
-            ev_counts = torch.cuda.Event()
-            ev_counts.record()
-            row0_dev = torch.empty((world * B + 1,), dtype=torch.int32, device=dev)
-            _lib.call("gs_xr_pack_dev", *pack_args, allc.data_ptr(), me, row0_dev.data_ptr(), cap, stream)
-            _t("x3 pack")
-            peer.barrier()
-            _t("x4 all_to_all")
-            global PIGGYBACK_OUT
-            cnt = _read_counts_on_side_stream(allc, ev_counts, (world, B, world))
-            PIGGYBACK_OUT = None if allp is None else _read_counts_on_side_stream(allp, ev_counts, (world, -1))
-            _t("x2 gather counts")
-        else:
-            cnt = gather_counts(counts.t().contiguous(), group)          # cnt[i][k][j]
-            _t("x2 gather counts")
+        flat =counts.t().contiguous().reshape(-1)                    # [camera k][destination j]
+        allc = torch.empty((world * flat.numel(),), dtype=torch.int32, device=dev)
+        dist.all_gather_into_tensor(allc, flat, group=group)          # cnt[i][k][j]
+        allp = _piggyback_gather(dev, world, group)
+        ev_counts = torch.cuda.Event()
+        ev_counts.record()
+        row0_dev = torch.empty((world * B + 1,), dtype=torch.int32, device=dev)
+        _lib.call("gs_xr_pack_dev", *pack_args, allc.data_ptr(), me, row0_dev.data_ptr(), cap, stream)
+        _t("x3 pack")
+        peer.barrier()
+        _t("x4 all_to_all")
+        global PIGGYBACK_OUT
+        cnt = _read_counts_on_side_stream(allc, ev_counts, (world, B, world))
+        PIGGYBACK_OUT = None if allp is None else _read_counts_on_side_stream(allp, ev_counts, (world, -1))
+        _t("x2 gather counts")
         c64 = np.asarray(cnt, dtype=np.int64)
-        if int(c64.sum(axis=(0, 1)).max()) <= peer.cap_rows:
-            row0, view_start = direct_rows(c64, me)       # decided from the all-gathered counts: identical on all ranks
-            row0_c = _i32(row0)
-            if not DEVICE_ROWS:
-                _lib.call("gs_xr_pack", *pack_args, row0_c, cap, stream)
-                _t("x3 pack")
-                peer.barrier()
-                _t("x4 all_to_all")
+        if peer.fits_direct(c64):   # decided from the all-gathered counts: identical on all ranks (k_xr_rows agrees)
+            row0, view_start = direct_rows(c64, me)
             state = dict(group=group, radii=radii, depths=depths, m2d=m2d, blkbase=blkbase, B=B, P=P, W=world, H=H,
-                         Wimg=Wimg, lo=lo_c, hi=hi_c, row0=row0_c, view_start=view_start, peer=peer, cnt=cnt, me=me,
+                         Wimg=Wimg, lo=lo_c, hi=hi_c, row0=_i32(row0), view_start=view_start, peer=peer, cnt=cnt, me=me,
                          keep=(rgb_c, co_c))
             res = _ExchangeSplatsDirect.apply(state, means2D, rgb, conic_opacity)
             return res, view_start, cnt
@@ -596,8 +539,7 @@ def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, setting
     view_start = [0]
     for n in layout.n_recv:
         view_start.append(view_start[-1] + n)
-    use_peer = peer is not None and peer.fits(cnt)   # decided from the all-gathered counts: identical on all ranks
     state = dict(layout=layout, group=group, radii=radii, depths=depths, flags=flags, gpos=gpos, B=B, P=P, W=world,
-                 segs=segments(layout), view_start=view_start, peer=peer if use_peer else None, cnt=cnt, me=me)
+                 segs=segments(layout), view_start=view_start)
     res = _ExchangeSplats.apply(state, means2D, rgb, conic_opacity)
     return res, view_start, cnt

@@ -142,9 +142,10 @@ class Trainer:
         max_sh_degree: the SH degree the model stores (GaussianParams)."""
         from . import exchange as _ex
         self._ex = _ex
-        # splat / gradient rows travel by direct NVLink stores from the pack kernels (exchange.PeerBuffers) instead of
-        # all_to_all_single; peer_exchange=None: on unless GS_B200_EXCHANGE=nccl.  Buffers hold peer_cap_rows rows
-        # (default 1.25 x the scene's Gaussians); a step that needs more falls back to all_to_all_single.
+        # splats travel by direct NVLink stores from the pack kernel and their gradients are pulled back over NVLink
+        # (exchange.PeerBuffers) instead of all_to_all_single; peer_exchange=None: on unless GS_B200_EXCHANGE=nccl.
+        # Buffers hold peer_cap_rows rows (default 1.25 x the scene's Gaussians); a step that needs more falls back to
+        # all_to_all_single.
         if peer_exchange is None:
             import os as _os
             peer_exchange = _os.environ.get("GS_B200_EXCHANGE", "p2p") != "nccl"

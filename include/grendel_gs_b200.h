@@ -326,10 +326,7 @@ enum {
     GS_DEBUG_BWD_TILE = 2,
     /* gs_render_forward: the half-warp-per-4x4-block blend kernel of round 1 (k_blend_fwd) instead of the packed
      * two-pixels-per-lane kernel (k_blend_fwd2); the images are bit-identical. */
-    GS_DEBUG_FWD_HALFWARP = 4,
-    /* direct exchange: pack with a CTA-level compaction per destination (one row per thread, 200-400-byte NVLink spans)
-     * instead of per-warp stores; same rows, same bytes (A/B switch until it is measured at 8 ranks) */
-    GS_DEBUG_XR_PACK_CTA = 8
+    GS_DEBUG_FWD_HALFWARP = 4
 };
 GS_API int gs_debug_set(int flags);
 
@@ -400,49 +397,29 @@ GS_API int gs_xchg_scatter_grad(int B, int P, int W, const uint8_t *flags, const
                                 void *const *d_means2D_ptrs_host, void *const *d_rgb_ptrs_host,
                                 void *const *d_conic_opacity_ptrs_host, void *stream);
 
-/* ---- the same exchange over NVLink peer memory: pack + transfer fused in one kernel -----------------------------
+/* ---- NVLink peer memory for the direct-placement exchange below ---------------------------------------------------
  * Replaces torch.distributed.all_to_all_single (gaussian_renderer/__init__.py:609-628 forward, its autograd mirror
- * backward) for ranks of one NVLink/NVSwitch node.  Each rank owns one receive buffer (11-float rows) and one
- * gradient buffer (9-float rows), allocated by gs_peer_alloc and exported as a 64-byte CUDA IPC handle; peers map
- * them with gs_peer_open.  gs_xchg_pack_p2p stores every row directly into its final row of the destination's
- * receive buffer (the row all_to_all_single would have delivered it to), gs_xchg_pack_grad_p2p stores every gradient
- * row directly into the row of the source's gradient buffer that gs_xchg_scatter_grad reads.  The caller orders
- * producers and consumers across ranks (a 4-byte all-reduce enqueued after the kernel; see csrc/distribute.cu). */
+ * backward) for ranks of one NVLink/NVSwitch node.  Each rank owns one receive region (11 * cap floats) and one
+ * gradient region (10 * cap floats), allocated by gs_peer_alloc and exported as a 64-byte CUDA IPC handle; peers map
+ * them with gs_peer_open.  gs_xr_pack_dev stores every splat directly into its final row of the destination's receive
+ * region, gs_xr_pull_grad loads every gradient row directly from the gradient regions of the ranks the splat was sent
+ * to.  The caller orders producers and consumers across ranks (a 4-byte all-reduce enqueued after the kernel; see
+ * csrc/distribute.cu). */
 GS_API int gs_peer_alloc(size_t bytes, void **dev_ptr, void *ipc_handle_64);
 GS_API int gs_peer_open(const void *ipc_handle_64, void **peer_ptr);
 GS_API int gs_peer_close(void *peer_ptr);
 GS_API int gs_peer_free(void *dev_ptr);
-/* dst_rows_ptrs_host: HOST array of W pointers, rank j's receive buffer as mapped in this process (own buffer for
- * j == me); row_delta_host: HOST (W) = recv_base_j[me] - send_base_me[j]. */
-GS_API int gs_xchg_pack_p2p(int B, int P, int W, const uint8_t *flags, const int32_t *gpos,
-                            const void *const *means2D_ptrs_host, const void *const *rgb_ptrs_host,
-                            const void *const *conic_opacity_ptrs_host, const void *const *radii_ptrs_host,
-                            const void *const *depths_ptrs_host, void *const *dst_rows_ptrs_host,
-                            const int32_t *row_delta_host, void *stream);
-/* seg_dst_ptrs_host: HOST array of nseg pointers, the first gradient row of segment q inside the SOURCE rank's
- * gradient buffer (as mapped in this process). */
-GS_API int gs_xchg_pack_grad_p2p(int nseg, const int32_t *seg_recv_start_host, const int32_t *seg_len_host,
-                                 const int32_t *seg_cam_host, const int32_t *seg_dst_start_host, int total_rows, int B,
-                                 const void *const *d_means2D_ptrs_host, const void *const *d_rgb_ptrs_host,
-                                 const void *const *d_conic_opacity_ptrs_host, void *const *seg_dst_ptrs_host,
-                                 void *stream);
 
-/* gs_xr_pack with the destination rows computed on the device from the all-gathered counts (counts_all_dev: W*B*W int32,
- * [source][camera][destination]; row0_dev: W*B + 1 int32 scratch = rows + over-capacity flag): enqueued right behind the
- * all-gather of gaussian_renderer/__init__.py:609-628's sizes, before the host has read them -- the stream does not run
- * dry at the exchange's host sync.  Over capacity nothing is written and every rank takes the all_to_all_single path. */
-GS_API int gs_xr_pack_dev(int B, int P, int W, int image_height, int image_width, const void *const *means2D_ptrs_host,
-                          const void *const *rgb_ptrs_host, const void *const *conic_opacity_ptrs_host,
-                          const void *const *radii_ptrs_host, const void *const *depths_ptrs_host,
-                          const int32_t *row_lo_host, const int32_t *row_hi_host, const int32_t *blkbase,
-                          void *const *peer_recv_ptrs_host, const int32_t *counts_all_dev, int me, int32_t *row0_dev,
-                          long long cap_rows, void *stream);
 /* ---- direct-placement exchange (csrc/distribute.cu, "xr"): same collective, same row order, but nothing is staged --
  * gs_xr_count: per (destination rank j, camera k, block of 256 splats) hit counts + their exclusive scan + the (j,k)
  * totals (the counts every rank all-gathers, gaussian_renderer/__init__.py:574-588).
- * gs_xr_pack: every splat is stored field by field into its FINAL row of the destination rank's structure-of-arrays
+ * gs_xr_pack_dev: every splat is stored field by field into its FINAL row of the destination rank's structure-of-arrays
  * receive region (means2D | rgb | conic_opacity | radii | depths, cap_rows rows each; gs_peer_alloc'ed, 11*cap floats),
  * i.e. straight into the tensors that rank's render reads -- no send rows, no unpack (replaces :590-607 and :631-658).
+ * The destination rows are computed on the device from the all-gathered counts (counts_all_dev: W*B*W int32,
+ * [source][camera][destination]; row0_dev: W*B + 1 int32 scratch = rows + over-capacity flag), so the pack is enqueued
+ * right behind the all-gather of :609-628's sizes, before the host has read them -- the stream does not run dry at the
+ * exchange's host sync.  Over capacity nothing is written and every rank takes the all_to_all_single path.
  * gs_xr_pull_grad: the mirrored backward; the owner of a splat loads its gradient rows from the gradient regions
  * (d means2D (2) | d rgb padded to 4 floats per row | d conic_opacity (4): 10*cap floats) of the ranks it sent the
  * splat to and sums them.
@@ -453,11 +430,12 @@ GS_API size_t gs_xr_temp_bytes(int B, int P, int W);
 GS_API int gs_xr_count(int B, int P, int W, int image_height, int image_width, const void *const *means2D_ptrs_host,
                        const void *const *radii_ptrs_host, const int32_t *row_lo_host, const int32_t *row_hi_host,
                        int32_t *blkcnt, int32_t *blkbase, int32_t *counts, void *temp, size_t temp_bytes, void *stream);
-GS_API int gs_xr_pack(int B, int P, int W, int image_height, int image_width, const void *const *means2D_ptrs_host,
-                      const void *const *rgb_ptrs_host, const void *const *conic_opacity_ptrs_host,
-                      const void *const *radii_ptrs_host, const void *const *depths_ptrs_host,
-                      const int32_t *row_lo_host, const int32_t *row_hi_host, const int32_t *blkbase,
-                      void *const *peer_recv_ptrs_host, const int32_t *dst_row0_host, long long cap_rows, void *stream);
+GS_API int gs_xr_pack_dev(int B, int P, int W, int image_height, int image_width, const void *const *means2D_ptrs_host,
+                          const void *const *rgb_ptrs_host, const void *const *conic_opacity_ptrs_host,
+                          const void *const *radii_ptrs_host, const void *const *depths_ptrs_host,
+                          const int32_t *row_lo_host, const int32_t *row_hi_host, const int32_t *blkbase,
+                          void *const *peer_recv_ptrs_host, const int32_t *counts_all_dev, int me, int32_t *row0_dev,
+                          long long cap_rows, void *stream);
 GS_API int gs_xr_pull_grad(int B, int P, int W, int image_height, int image_width, const void *const *means2D_ptrs_host,
                            const void *const *radii_ptrs_host, const int32_t *row_lo_host, const int32_t *row_hi_host,
                            const int32_t *blkbase, void *const *peer_grad_ptrs_host, const int32_t *dst_row0_host,

@@ -76,8 +76,8 @@ def test_argument_errors_are_reported_not_crashed(lib):
         ("gs_render_count_read", (ctypes.cast(ctypes.byref(R), vp), ctypes.byref(R), None)),   # not a ticket of the library
         ("gs_render_backward_batched", (0, 0, 0, 16, 16, None, None, None, None, None, None, None, None, None, 0, None, None, None, None)),
         ("gs_loss_forward_batched", (1, 16, 16, None, None, None, None, None, 0, None)),
-        ("gs_xchg_pack_p2p", (0, 4, 2, None, None, None, None, None, None, None, None, None, None)),
-        ("gs_xchg_pack_grad_p2p", (1, None, None, None, None, 8, 1, None, None, None, None, None)),
+        ("gs_xr_pack_dev", (0, 4, 2, 16, 16, None, None, None, None, None, None, None, None, None, None, 0, None, 64, None)),
+        ("gs_xr_pull_grad", (1, 4, 17, 16, 16, None, None, None, None, None, None, None, 64, None, None, None, None)),
         ("gs_peer_alloc", (0, None, None)),
         ("gs_peer_open", (None, None)),
         ("gs_adam_step", (9, None, None, None, None, None, None, None, None, None, None, ctypes.c_float(1.0), None)),

@@ -2,11 +2,10 @@
 GPU, against the numpy reference of tests/exchange_ref.py.
 
 No kernel knows whether a destination pointer is a peer's IPC mapping or an ordinary allocation on the same device: all
-cross-rank state enters through host tables (strip rows, destination rows, row deltas, segment tables) or one device
-array of all-gathered counts.  So every rank's receive and gradient regions are plain allocations here, and every
+cross-rank state enters through host tables (strip rows, destination rows, segment tables) or one device array of
+all-gathered counts.  So every rank's receive and gradient regions are plain allocations here, and every
 collective is a host-side concatenation or split.  Kernel arguments are built with exchange.py's own helpers (_slab_ptrs,
-_row_ptrs, _i32, direct_rows, peer_row_deltas, peer_grad_rows, Layout, segments), so the product's glue is under test
-as well.  What stays with tests/mgpu_parity.py: IPC mapping, NCCL, and the ordering of ranks' streams.
+_row_ptrs, _i32, direct_rows, Layout, segments), so the product's glue is under test as well.  What stays with tests/mgpu_parity.py: IPC mapping, NCCL, and the ordering of ranks' streams.
 
 Every output lives in a slab filled with 0xFF bytes, with guard bands around each region: a stray write shows up as a
 changed sentinel.  The exchange copies and sums in a fixed order, so all comparisons are bit for bit (int32 views)."""
@@ -153,7 +152,7 @@ def get_case(name):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# direct placement (the live path): count -> pack / pack_dev (both pack kernels) -> pull_grad
+# direct placement (the peer-memory path): count -> pack_dev -> pull_grad
 # ---------------------------------------------------------------------------------------------------------------------
 def xr_count(c, i):
     B, P, W = c.B, c.P[i], c.W
@@ -172,21 +171,16 @@ def pack_args(c, i, blkbase, bases):
             c.ptrs(i, "radii"), c.ptrs(i, "depths"), c.lo_c, c.hi_c, blkbase.data_ptr(), bases)
 
 
-def run_pack(c, blkbases, cap, allc=None):
-    """Every simulated rank packs into the W receive regions (host rows, or device rows from `allc`).
-    -> (region slab, row0_dev slab or None)."""
+def run_pack(c, blkbases, cap, allc):
+    """Every simulated rank packs into the W receive regions, its destination rows computed on the device from the
+    all-gathered counts `allc`.  -> (region slab, row0_dev slab)."""
     W, B = c.W, c.B
     slab = Slab([4 * 11 * cap] * W)
     bases = (C.c_void_p * W)(*[slab.regions[j].data_ptr() for j in range(W)])
-    rows = Slab([4 * (W * B + 1)] * W) if allc is not None else None
+    rows = Slab([4 * (W * B + 1)] * W)
     for i in range(W):
-        args = pack_args(c, i, blkbases[i], bases)
-        if allc is None:
-            row0, _ = exchange.direct_rows(c.cnt, i)
-            _lib.call("gs_xr_pack", *args, _i32(row0), C.c_longlong(cap), gu.stream())
-        else:
-            _lib.call("gs_xr_pack_dev", *args, allc.data_ptr(), i, rows.regions[i].data_ptr(), C.c_longlong(cap),
-                      gu.stream())
+        _lib.call("gs_xr_pack_dev", *pack_args(c, i, blkbases[i], bases), allc.data_ptr(), i, rows.regions[i].data_ptr(),
+                  C.c_longlong(cap), gu.stream())
     return slab, rows
 
 
@@ -216,37 +210,21 @@ def test_exchange_sim_direct_placement(name):
         assert slab.guards_intact()
         blk.append((counts, blkbase))
     blkbases = [b for _, b in blk]
-    # 2. pack with host rows
+    # 2. pack with device rows from the all-gathered counts, laid out as exchange_cat's all_gather leaves them
     cap = (max(c.N) // 4 + 2) * 4
-    host, _ = run_pack(c, blkbases, cap)
-    check_regions(c, host, cap)
-    ref_words = [host.words(j) for j in range(W)]
-    # 3. pack with device rows from the all-gathered counts, laid out as exchange_cat's all_gather leaves them
     allc = torch.cat([counts.t().contiguous().reshape(-1) for counts, _ in blk])
     devp, rows = run_pack(c, blkbases, cap, allc)
     for me in range(W):
         r = rows.words(me)
         assert r[:W * B].tolist() == exchange.direct_rows(c.cnt, me)[0] and r[W * B] == 0, f"rank {me}: device rows"
-    assert rows.guards_intact() and devp.guards_intact()
-    assert all(np.array_equal(devp.words(j), ref_words[j]) for j in range(W))
+    assert rows.guards_intact()
+    check_regions(c, devp, cap)
     small = (max(c.N) - 1) // 4 * 4           # a positive multiple of 4 below the largest receiver total
     if small > 0:
         over, rows = run_pack(c, blkbases, small, allc)
         assert all(rows.words(me)[W * B] == 1 for me in range(W)), "over-capacity flag"
         assert bool((over.buf == 0xFF).all()), "an over-capacity pack wrote rows"
-    # 4. the CTA-compacted pack kernel: bit-identical regions
-    prev = _lib.debug_set(_lib.DEBUG_XR_PACK_CTA)
-    try:
-        for allc_ in (None, allc):
-            cta, _ = run_pack(c, blkbases, cap, allc_)
-            assert cta.guards_intact()
-            assert all(np.array_equal(cta.words(j), ref_words[j]) for j in range(W)), "CTA pack differs"
-        if small > 0:
-            over, _ = run_pack(c, blkbases, small, allc)
-            assert bool((over.buf == 0xFF).all()), "an over-capacity CTA pack wrote rows"
-    finally:
-        _lib.debug_set(prev)
-    # 5. pull the gradients back: sum over the destinations in ascending rank order.  The padding float of the 16-byte
+    # 3. pull the gradients back: sum over the destinations in ascending rank order.  The padding float of the 16-byte
     #    d rgb rows is NaN and rows beyond N_j keep the NaN fill: neither may reach a source's gradient.
     grad = Slab([4 * 10 * cap] * W)
     for j in range(W):
@@ -276,8 +254,8 @@ def test_exchange_sim_direct_placement(name):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# row-staged and peer-row paths (the fallback): route -> pack -> all-to-all -> unpack, pack_p2p; pack_grad (+ p2p) ->
-# reverse all-to-all -> scatter_grad
+# row staging over NCCL (the fallback): route -> pack -> all-to-all -> unpack; pack_grad -> reverse all-to-all ->
+# scatter_grad
 # ---------------------------------------------------------------------------------------------------------------------
 def staged_grad_rows(c, j):
     """Receiver j's expected 9-float gradient rows in its row-staged receive order (g_eff)."""
@@ -297,7 +275,7 @@ def test_exchange_sim_row_staged(name):
     W, B, s = c.W, c.B, gu.stream()
     # the segment table of gs_xchg_unpack / pack_grad holds MAX_SEGMENTS non-empty (source, camera) blocks
     nseg = [int((c.cnt[:, :, j] > 0).sum()) for j in range(W)]
-    # 6. route: flags [j][k][i], their exclusive scan, counts [j][k]
+    # 4. route: flags [j][k][i], their exclusive scan, counts [j][k]
     routed, sends = [], []
     for i in range(W):
         P = c.P[i]
@@ -314,7 +292,7 @@ def test_exchange_sim_row_staged(name):
             assert np.array_equal(f, c.hits[i].transpose(2, 0, 1).astype(np.uint8)), f"rank {i}: flags"
             e = f.reshape(-1).astype(np.int64)
             assert np.array_equal(gu.npy(gpos).astype(np.int64), np.cumsum(e) - e), f"rank {i}: gpos"
-        # 7. pack: the 11-float send rows in all_to_all_single order
+        # 5. pack: the 11-float send rows in all_to_all_single order
         T = c.layouts[i].total_send
         send = slab.f32(3, (-1, exchange.ROW))
         _lib.call("gs_xchg_pack", B, P, W, flags.data_ptr(), gpos.data_ptr(), c.ptrs(i, "means2D"), c.ptrs(i, "rgb"),
@@ -330,7 +308,7 @@ def test_exchange_sim_row_staged(name):
         parts = [sends[i].split(c.layouts[i].send_splits)[j] for i in range(W)]
         assert [p.shape[0] for p in parts] == c.layouts[j].recv_splits
         recv.append(torch.cat(parts).contiguous())
-    # 7. unpack on every receiver: the reference outputs (== the direct placement's regions)
+    # 6. unpack on every receiver: the reference outputs (== the direct placement's regions)
     for j in range(W):
         lay, n = c.layouts[j], c.N[j]
         vs = [int(v) for v in c.ref.view[j]]
@@ -342,7 +320,7 @@ def test_exchange_sim_row_staged(name):
                 _row_ptrs(out.f32(2, (n, 4)), vs, B), _row_ptrs(out.i32(3, (n,)), vs, B), _row_ptrs(out.f32(4, (n,)), vs, B),
                 s)
         if nseg[j] > exchange.MAX_SEGMENTS:
-            # 10. more (source, camera) blocks than the segment table holds: a clean error, nothing launched
+            # 8. more (source, camera) blocks than the segment table holds: a clean error, nothing launched
             with pytest.raises(_lib.GsError, match="segments"):
                 _lib.call("gs_xchg_unpack", *args)
             torch.cuda.synchronize()
@@ -352,19 +330,7 @@ def test_exchange_sim_row_staged(name):
         assert out.guards_intact()
         for q, f in enumerate(xr.FIELDS):
             assert same(bits(gu.npy(o[q])), bits(c.outputs[j][f]).reshape(-1)), f"receiver {j}: {f}"
-    # 8. pack_p2p straight into the W receive buffers: the simulated all-to-all's buffers
-    rbuf = Slab([4 * max(n, 0) * exchange.ROW for n in c.N])
-    dst = (C.c_void_p * W)(*[rbuf.regions[j].data_ptr() for j in range(W)])
-    for i in range(W):
-        flags, gpos, _ = routed[i]
-        _lib.call("gs_xchg_pack_p2p", B, c.P[i], W, flags.data_ptr(), gpos.data_ptr(), c.ptrs(i, "means2D"),
-                  c.ptrs(i, "rgb"), c.ptrs(i, "conic_opacity"), c.ptrs(i, "radii"), c.ptrs(i, "depths"), dst,
-                  _i32(exchange.peer_row_deltas(c.cnt, i)), s)
-    assert rbuf.guards_intact()
-    for j in range(W):
-        assert np.array_equal(rbuf.words(j), bits(gu.npy(recv[j])).reshape(-1)), f"receiver {j}: p2p rows"
-    # 9. backward: pack_grad (one camera NULL -> zeros), its peer form into the sources' buffers, scatter_grad
-    gsrc = Slab([4 * c.layouts[i].total_send * exchange.GROW for i in range(W)])
+    # 7. backward: pack_grad (one camera NULL -> zeros), the reverse all-to-all, scatter_grad
     grecv = []
     for j in range(W):
         lay, n = c.layouts[j], c.N[j]
@@ -380,14 +346,9 @@ def test_exchange_sim_row_staged(name):
         rs, ln, cam, ds = exchange.segments(lay)
         rows_out = Slab([4 * n * exchange.GROW])
         args = (len(rs), _i32(rs), _i32(ln), _i32(cam), _i32(ds), lay.total_recv, B, *gp)
-        grow = exchange.peer_grad_rows(c.cnt, j)
-        seg_dst = (C.c_void_p * len(rs))(*[gsrc.regions[q // B].data_ptr() + grow[q] * exchange.GROW * 4
-                                           for q in range(len(rs))])
         if nseg[j] > exchange.MAX_SEGMENTS:
             with pytest.raises(_lib.GsError, match="segments"):
                 _lib.call("gs_xchg_pack_grad", *args, rows_out.regions[0].data_ptr(), s)
-            with pytest.raises(_lib.GsError, match="segments"):
-                _lib.call("gs_xchg_pack_grad_p2p", *args, seg_dst, s)
             torch.cuda.synchronize()
             assert bool((rows_out.buf == 0xFF).all())
             continue
@@ -395,21 +356,22 @@ def test_exchange_sim_row_staged(name):
         got = gu.npy(rows_out.f32(0, (n, exchange.GROW)))
         assert rows_out.guards_intact() and same(got, staged_grad_rows(c, j)), f"receiver {j}: gradient rows"
         grecv.append(rows_out.f32(0, (n, exchange.GROW)))
-        _lib.call("gs_xchg_pack_grad_p2p", *args, seg_dst, s)
     if max(nseg) > exchange.MAX_SEGMENTS:
         return      # the row-staged path cannot serve this step; the direct placement test covers its backward
-    assert gsrc.guards_intact()
     for i in range(W):
-        gsend = torch.cat([grecv[j].split(c.layouts[j].recv_splits)[i] for j in range(W)])
-        assert np.array_equal(gsrc.words(i), bits(gu.npy(gsend)).reshape(-1)), f"rank {i}: p2p gradient rows"
+        # the reverse all-to-all, simulated: rank i receives its block of every receiver's gradient rows, in rank order
+        # (at least one row, as _ExchangeSplats allocates it: a zero-size buffer has no address)
+        T = c.layouts[i].total_send
+        gsend = Slab([4 * max(T, 1) * exchange.GROW])
+        gsend.f32(0, (-1, exchange.GROW))[:T] = torch.cat([grecv[j].split(c.layouts[j].recv_splits)[i]
+                                                           for j in range(W)])
         P = c.P[i]
         flags, gpos, _ = routed[i]
         out = Slab([4 * B * P * xr.WIDTH[f] for f in xr.GRAD_FIELDS])
         d = [out.f32(q, (B, P, xr.WIDTH[f])) for q, f in enumerate(xr.GRAD_FIELDS)]
-        # the scatter reads the rows gs_xchg_pack_grad_p2p stored into this rank's gradient buffer (== gsend)
-        _lib.call("gs_xchg_scatter_grad", B, P, W, flags.data_ptr(), gpos.data_ptr(), gsrc.regions[i].data_ptr(),
+        _lib.call("gs_xchg_scatter_grad", B, P, W, flags.data_ptr(), gpos.data_ptr(), gsend.regions[0].data_ptr(),
                   _slab_ptrs(d[0], B), _slab_ptrs(d[1], B), _slab_ptrs(d[2], B), s)
-        assert out.guards_intact()
+        assert out.guards_intact() and gsend.guards_intact()
         for q, f in enumerate(xr.GRAD_FIELDS):
             got = gu.npy(d[q])
             assert same(got, c.back[i][f]), f"rank {i}: d {f}"
