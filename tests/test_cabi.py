@@ -157,6 +157,56 @@ def test_preprocess_argument_checks(lib):
         assert rc["P 0, no image"] == (-1 if name == "gs_preprocess_forward" else 0), name
 
 
+LOSS_ARGS = r"""
+import ctypes, json, sys
+sys.path.insert(0, %(pkg)r)
+from gs_b200 import _lib
+lib = _lib.load()
+FAKE = 1 << 20   # an address that is never dereferenced: no device is visible to this process
+H, W = 64, 16
+
+def call(rows, gts=None, B=None, temp_bytes=None):
+    B = len(rows) if B is None else B
+    flat = (ctypes.c_int32 * max(4, 4 * len(rows)))(*[v for r in rows for v in r])
+    g = (ctypes.c_void_p * max(1, len(rows)))(*(gts if gts is not None else [FAKE] * len(rows)))
+    tb = lib.gs_loss_temp_bytes_batched(len(rows), flat, W) if temp_bytes is None else temp_bytes
+    f = lib.gs_loss_forward_batched(B, H, W, flat, FAKE, g, FAKE, FAKE, tb, None)
+    b = lib.gs_loss_backward_batched(B, H, W, flat, FAKE, g, FAKE, FAKE, FAKE, FAKE, None)
+    return [f, b]
+
+ok = (0, 32, 5, 27)
+maps = 1024 + 9 * 32 * W * 4
+print(json.dumps({
+    "B 0": call([ok], B=0), "B 65": call([ok] * 65),
+    "row0 < 0": call([(-1, 32, 0, 32)]), "row1 > H": call([(0, H + 1, 0, H)]), "row1 < row0": call([(9, 8, 8, 8)]),
+    "c0 < row0": call([(8, 32, 7, 32)]), "c1 > row1": call([(0, 32, 0, 33)]), "c1 < c0": call([(0, 32, 20, 19)]),
+    "null gt": call([(0, 0, 0, 0), ok], gts=[None, None]), "null gt, second view": call([ok, ok], gts=[FAKE, None]),
+    "one byte short": call([ok], temp_bytes=maps - 1),
+    "valid": call([ok], temp_bytes=maps), "valid, empty view without gt": call([(0, 0, 0, 0), ok], gts=[None, FAKE]),
+}))
+"""
+
+
+def test_loss_argument_checks(lib):
+    """gs_loss_{forward,backward}_batched refuse bad view counts, rows and ground-truth pointers before any launch, and
+    the forward a workspace one byte short of the header and maps.  The calls run in a process that sees no device, so
+    a check that stops working ends in a launch error and never touches one."""
+    import json
+    import subprocess
+    import sys
+    code = LOSS_ARGS % dict(pkg=os.path.join(ROOT, "grendel-gs_b200"))
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300,
+                       env=dict(os.environ, CUDA_VISIBLE_DEVICES=""))
+    assert r.returncode == 0, r.stderr[-3000:]
+    out = json.loads(r.stdout.strip().splitlines()[-1])
+    for case in ("B 0", "B 65", "row0 < 0", "row1 > H", "row1 < row0", "c0 < row0", "c1 > row1", "c1 < c0", "null gt",
+                 "null gt, second view"):
+        assert out[case] == [-1, -1], (case, out[case])                   # GS_EINVAL, forward and backward
+    assert out["one byte short"][0] == -3                                  # GS_ENOMEM; the backward takes no size
+    for case in ("valid", "valid, empty view without gt"):
+        assert out[case] == [-2, -2], (case, out[case])                   # GS_ECUDA: passed every check, no device
+
+
 def test_dropin_package_exports_reference_names():
     import diff_gaussian_rasterization as d
     from simple_knn._C import distCUDA2  # noqa: F401

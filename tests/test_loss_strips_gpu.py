@@ -74,25 +74,6 @@ def kernel_loss(img, gt, r0, r1, c0, c1, x=None):
     return float(l1), float(ss), x
 
 
-def check_vs_fp64(tag, got, ref32, ref64):
-    """Scalars and gradient no farther from fp64 than the fp32 oracle's evaluation of the same loss.
-
-    The gradient is judged by its worst error, err / (|ref| + rms(ref)), not by the count of entries past the 1e-4 bar.
-    Near-flat windows (the flat ground-truth and image regions) make sigma^2 = E[x^2] - mu^2 a cancellation of two
-    numbers ~1 down to ~1e-7 next to C2 = 9e-4, so EVERY fp32 evaluation's gradient there is ~1e-4 relative off fp64:
-    right at the bar, and how many entries land past it depends on the summation order (the kernel's separable row /
-    column passes vs the oracle's), not on correctness.  Measured on an H100: kernel worst 2.4e-4 against the oracle's
-    1.8e-4, with up to 0.9 % of the kernel's entries past 1e-4 (0.07 % of the oracle's).  A wrong weight, row or tile
-    edge moves the worst error by orders of magnitude."""
-    (gl1, gss, gg), (ol1, oss, og), (rl1, rss, rg) = got, ref32, ref64
-    for name, k, o, r in (("Ll1", gl1, ol1, rl1), ("ssim", gss, oss, rss)):
-        assert abs(k - r) <= 2 * abs(o - r) + 1e-6 * abs(r) + 1e-9, (tag, name, k, o, r)
-    gu.floor_report(tag + ".grad", gg, og, rg)
-    _, mine = gu.outside(gg, rg)
-    _, floor = gu.outside(og, rg)
-    assert mine <= 2.0 * floor + 1e-6, (tag, mine, floor)
-
-
 @pytest.mark.parametrize("H,W,cuts", SHAPES)
 def test_loss_halo_strips_add_up_to_the_full_image(o32, H, W, cuts):
     img, gt = make_pair(H, W, seed=H * 1000 + W)
@@ -130,8 +111,8 @@ def test_loss_halo_strips_add_up_to_the_full_image(o32, H, W, cuts):
     gtf = np.clip(gt.astype(np.float32) / np.float32(255), 0, 1)
     ref32 = o32.loss(img, gtf, H * W, LAMBDA)
     ref64 = fp64_reference(img, gt, (0, H), H * W)
-    check_vs_fp64(f"strips {H}x{W} full", (l1_full, ss_full, g_full), ref32, ref64)
-    check_vs_fp64(f"strips {H}x{W} summed", (l1_sum, ss_sum, g_sum), ref32, ref64)
+    gu.check_vs_fp64(f"strips {H}x{W} full", (l1_full, ss_full, g_full), ref32, ref64)
+    gu.check_vs_fp64(f"strips {H}x{W} summed", (l1_sum, ss_sum, g_sum), ref32, ref64)
 
 
 @pytest.mark.parametrize("H,W,cuts", SHAPES)
@@ -148,5 +129,5 @@ def test_loss_edge_shapes_vs_fp64(o32, H, W, cuts):
         ol1, oss, og = o32.loss(img[:, r0:r1], gtf, H * W, LAMBDA)
         og_full = np.zeros(img.shape, np.float32)
         og_full[:, r0:r1] = og
-        check_vs_fp64(f"strip [{r0},{r1}) of {H}x{W}", (l1, ss, g), (ol1, oss, og_full),
-                      fp64_reference(img, gt, (r0, r1), H * W))
+        gu.check_vs_fp64(f"strip [{r0},{r1}) of {H}x{W}", (l1, ss, g), (ol1, oss, og_full),
+                         fp64_reference(img, gt, (r0, r1), H * W))
