@@ -356,21 +356,22 @@ extern "C" size_t gs_render_sort_temp_bytes(int64_t R) {
 // Implemented in blend.cu
 int gs_launch_blend_forward(int num_views, int64_t R, int H, int W, const float *rec, const float *bg,
                             const uint8_t *compute_locally, const uint32_t *ranges, const uint32_t *ids_sorted,
-                            float *image, float *final_T, uint32_t *n_contrib, int64_t *stats, void *seg_ws,
-                            size_t seg_ws_bytes, cudaStream_t stream);
+                            float *image, float *final_T, uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats,
+                            void *seg_ws, size_t seg_ws_bytes, cudaStream_t stream);
 
-extern "C" int gs_render_forward_batched(int num_views, const int32_t *view_start, int64_t R, int image_height,
-                                         int image_width, const float *means2D, const int32_t *radii,
-                                         const uint8_t *compute_locally, const uint32_t *order, const uint32_t *offsets,
-                                         const float *rec, const float *bg, uint32_t *tiles_unsorted,
-                                         uint32_t *ids_unsorted, uint32_t *tiles_sorted, uint32_t *ids_sorted,
-                                         void *sort_temp, size_t sort_temp_bytes, uint32_t *ranges, float *image,
-                                         float *final_T, uint32_t *n_contrib, int64_t *stats, void *seg_ws,
-                                         size_t seg_ws_bytes, void *stream_) {
+extern "C" int gs_render_forward_batched_ts(int num_views, const int32_t *view_start, int64_t R, int image_height,
+                                            int image_width, const float *means2D, const int32_t *radii,
+                                            const uint8_t *compute_locally, const uint32_t *order, const uint32_t *offsets,
+                                            const float *rec, const float *bg, uint32_t *tiles_unsorted,
+                                            uint32_t *ids_unsorted, uint32_t *tiles_sorted, uint32_t *ids_sorted,
+                                            void *sort_temp, size_t sort_temp_bytes, uint32_t *ranges, float *image,
+                                            float *final_T, uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats,
+                                            void *seg_ws, size_t seg_ws_bytes, void *stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     GS_REQUIRE(R >= 0 && image_height > 0 && image_width > 0, "sizes");
     GS_REQUIRE(R < (1ll << 31), "more than 2^31 splat-tile instances");
     GS_REQUIRE(compute_locally && bg && ranges && image && final_T && n_contrib, "null pointer");
+    GS_REQUIRE(((uintptr_t)tile_stats & 7) == 0, "tile_stats must be 8-byte aligned");
     const int gx = (image_width + GS_BLOCK_X - 1) / GS_BLOCK_X, gy = (image_height + GS_BLOCK_Y - 1) / GS_BLOCK_Y;
     GsViews views;
     {
@@ -408,7 +409,36 @@ extern "C" int gs_render_forward_batched(int num_views, const int32_t *view_star
         }
     }
     return gs_launch_blend_forward(num_views, R, image_height, image_width, rec, bg, compute_locally, ranges, ids_sorted,
-                                   image, final_T, n_contrib, stats, seg_ws, seg_ws_bytes, stream);
+                                   image, final_T, n_contrib, stats, tile_stats, seg_ws, seg_ws_bytes, stream);
+}
+
+extern "C" int gs_render_forward_batched(int num_views, const int32_t *view_start, int64_t R, int image_height,
+                                         int image_width, const float *means2D, const int32_t *radii,
+                                         const uint8_t *compute_locally, const uint32_t *order, const uint32_t *offsets,
+                                         const float *rec, const float *bg, uint32_t *tiles_unsorted,
+                                         uint32_t *ids_unsorted, uint32_t *tiles_sorted, uint32_t *ids_sorted,
+                                         void *sort_temp, size_t sort_temp_bytes, uint32_t *ranges, float *image,
+                                         float *final_T, uint32_t *n_contrib, int64_t *stats, void *seg_ws,
+                                         size_t seg_ws_bytes, void *stream) {
+    return gs_render_forward_batched_ts(num_views, view_start, R, image_height, image_width, means2D, radii,
+                                        compute_locally, order, offsets, rec, bg, tiles_unsorted, ids_unsorted,
+                                        tiles_sorted, ids_sorted, sort_temp, sort_temp_bytes, ranges, image, final_T,
+                                        n_contrib, stats, nullptr, seg_ws, seg_ws_bytes, stream);
+}
+
+extern "C" int gs_render_forward_ts(int P, int64_t R, int image_height, int image_width, const float *means2D,
+                                    const int32_t *radii, const uint8_t *compute_locally, const uint32_t *order,
+                                    const uint32_t *offsets, const float *rec, const float *bg, uint32_t *tiles_unsorted,
+                                    uint32_t *ids_unsorted, uint32_t *tiles_sorted, uint32_t *ids_sorted, void *sort_temp,
+                                    size_t sort_temp_bytes, uint32_t *ranges, float *image, float *final_T,
+                                    uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats, void *seg_ws,
+                                    size_t seg_ws_bytes, void *stream) {
+    GS_REQUIRE(P >= 0, "sizes");
+    const int32_t one_view[2] = {0, P};
+    return gs_render_forward_batched_ts(1, one_view, R, image_height, image_width, means2D, radii, compute_locally,
+                                        order, offsets, rec, bg, tiles_unsorted, ids_unsorted, tiles_sorted, ids_sorted,
+                                        sort_temp, sort_temp_bytes, ranges, image, final_T, n_contrib, stats, tile_stats,
+                                        seg_ws, seg_ws_bytes, stream);
 }
 
 extern "C" int gs_render_forward(int P, int64_t R, int image_height, int image_width, const float *means2D,
@@ -417,9 +447,7 @@ extern "C" int gs_render_forward(int P, int64_t R, int image_height, int image_w
                                  uint32_t *ids_unsorted, uint32_t *tiles_sorted, uint32_t *ids_sorted, void *sort_temp,
                                  size_t sort_temp_bytes, uint32_t *ranges, float *image, float *final_T,
                                  uint32_t *n_contrib, int64_t *stats, void *seg_ws, size_t seg_ws_bytes, void *stream) {
-    GS_REQUIRE(P >= 0, "sizes");
-    const int32_t one_view[2] = {0, P};
-    return gs_render_forward_batched(1, one_view, R, image_height, image_width, means2D, radii, compute_locally, order,
-                                     offsets, rec, bg, tiles_unsorted, ids_unsorted, tiles_sorted, ids_sorted, sort_temp,
-                                     sort_temp_bytes, ranges, image, final_T, n_contrib, stats, seg_ws, seg_ws_bytes, stream);
+    return gs_render_forward_ts(P, R, image_height, image_width, means2D, radii, compute_locally, order, offsets, rec, bg,
+                                tiles_unsorted, ids_unsorted, tiles_sorted, ids_sorted, sort_temp, sort_temp_bytes, ranges,
+                                image, final_T, n_contrib, stats, nullptr, seg_ws, seg_ws_bytes, stream);
 }

@@ -182,12 +182,21 @@ extern "C" size_t gs_render_seg_bytes(int64_t R, int num_tiles) { return seg_byt
 #ifndef FW_MIN_CTAS
 #define FW_MIN_CTAS 6
 #endif
-template <bool STATS, bool CKPT>
+// Per-tile statistics (gs_render_forward_ts): a forward instantiated with ONE trailing TileOut argument also stores the
+// CTA's own (list length, walked, blended) in row blockIdx.x of that (B*T, 3) array, and stats may then be NULL.  With an
+// empty pack the parameter list and the code are exactly those of the forms without per-tile statistics, whose SASS stays
+// the same instruction for instruction (cuobjdump -sass).  Keep the flag as `if constexpr (sizeof...(TileOut) != 0)`:
+// a local constexpr bool standing for it already changed nvcc's register numbering and ptxas' schedule of those forms.
+GS_D unsigned long long *tile_out() { return nullptr; }
+GS_D unsigned long long *tile_out(unsigned long long *p) { return p; }
+
+template <bool STATS, bool CKPT, typename... TileOut>
 __global__ void __launch_bounds__(BL_THREADS, FW_MIN_CTAS)
 k_blend_fwd(int W, int H, int tiles_per_view, const float4 *__restrict__ rec, const float *__restrict__ bg,
             const uint8_t *__restrict__ compute_locally, const uint2 *__restrict__ ranges,
             const uint32_t *__restrict__ ids, float *__restrict__ image, float *__restrict__ final_T,
-            uint32_t *__restrict__ n_contrib, unsigned long long *__restrict__ stats, const SegWs seg) {
+            uint32_t *__restrict__ n_contrib, unsigned long long *__restrict__ stats, const SegWs seg,
+            TileOut... tile_arg) {
     __shared__ SRec s_rec[FW_CHUNK];
     __shared__ uint16_t s_cull[FW_CHUNK];
     __shared__ unsigned long long s_stats[3];
@@ -207,6 +216,8 @@ k_blend_fwd(int W, int H, int tiles_per_view, const float4 *__restrict__ rec, co
     if (!compute_locally[blockIdx.x]) {  // non-local tiles must read exactly 0 (loss_distribution.py:1875)
         if (inside) { image[pix] = 0.f; image[HW + pix] = 0.f; image[2 * HW + pix] = 0.f; }
         if (CKPT && threadIdx.x == 0) seg.tile_last[blockIdx.x] = 0u;
+        if constexpr (sizeof...(TileOut) != 0)
+            if (threadIdx.x < 3) tile_out(tile_arg...)[3 * (size_t)blockIdx.x + threadIdx.x] = 0ull;
         return;
     }
     const uint2 range = ranges[blockIdx.x];
@@ -333,7 +344,15 @@ k_blend_fwd(int W, int H, int tiles_per_view, const float4 *__restrict__ rec, co
         }
         if (lane == 0) { atomicAdd(&s_stats[0], v0); atomicAdd(&s_stats[1], v1); atomicAdd(&s_stats[2], v2); }
         __syncthreads();
-        if (threadIdx.x < 3) atomicAdd(&stats[3 * view + threadIdx.x], s_stats[threadIdx.x]);
+        if constexpr (sizeof...(TileOut) != 0) {   // this CTA's row: list length, walked, blended
+            if (threadIdx.x < 3) {
+                if (stats) atomicAdd(&stats[3 * view + threadIdx.x], s_stats[threadIdx.x]);
+                tile_out(tile_arg...)[3 * (size_t)blockIdx.x + threadIdx.x] =
+                    threadIdx.x ? s_stats[threadIdx.x] : (unsigned long long)total;
+            }
+        } else {
+            if (threadIdx.x < 3) atomicAdd(&stats[3 * view + threadIdx.x], s_stats[threadIdx.x]);
+        }
     }
 }
 
@@ -364,12 +383,13 @@ GS_D p2 p2_add(p2 a, p2 b) { return {__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi
 GS_D void p2_fma_acc(p2 &c, p2 a, p2 b) { c = p2_fma(a, b, c); }
 GS_D void p2_mul_acc(p2 &t, p2 f) { t = p2_mul(t, f); }
 
-template <bool STATS, bool CKPT>
+template <bool STATS, bool CKPT, typename... TileOut>   // TileOut: see k_blend_fwd
 __global__ void __launch_bounds__(F2_THREADS, F2_MIN_CTAS)
 k_blend_fwd2(int W, int H, int tiles_per_view, const float4 *__restrict__ rec, const float *__restrict__ bg,
              const uint8_t *__restrict__ compute_locally, const uint2 *__restrict__ ranges,
              const uint32_t *__restrict__ ids, float *__restrict__ image, float *__restrict__ final_T,
-             uint32_t *__restrict__ n_contrib, unsigned long long *__restrict__ stats, const SegWs seg) {
+             uint32_t *__restrict__ n_contrib, unsigned long long *__restrict__ stats, const SegWs seg,
+             TileOut... tile_arg) {
     __shared__ SRec s_rec[FW_CHUNK + 1];   // + the slot an empty candidate list points at (entry g0 + 32 of the last group)
     __shared__ uint16_t s_cull[FW_CHUNK];
     __shared__ unsigned long long s_stats[3];
@@ -390,6 +410,8 @@ k_blend_fwd2(int W, int H, int tiles_per_view, const float4 *__restrict__ rec, c
         if (in0) { image[pix] = 0.f; image[HW + pix] = 0.f; image[2 * HW + pix] = 0.f; }
         if (in1) { image[pix + 1] = 0.f; image[HW + pix + 1] = 0.f; image[2 * HW + pix + 1] = 0.f; }
         if (CKPT && threadIdx.x == 0) seg.tile_last[blockIdx.x] = 0u;
+        if constexpr (sizeof...(TileOut) != 0)
+            if (threadIdx.x < 3) tile_out(tile_arg...)[3 * (size_t)blockIdx.x + threadIdx.x] = 0ull;
         return;
     }
     const uint2 range = ranges[blockIdx.x];
@@ -550,7 +572,15 @@ k_blend_fwd2(int W, int H, int tiles_per_view, const float4 *__restrict__ rec, c
         }
         if (lane == 0) { atomicAdd(&s_stats[0], v0); atomicAdd(&s_stats[1], v1); atomicAdd(&s_stats[2], v2); }
         __syncthreads();
-        if (threadIdx.x < 3) atomicAdd(&stats[3 * view + threadIdx.x], s_stats[threadIdx.x]);
+        if constexpr (sizeof...(TileOut) != 0) {   // this CTA's row: list length, walked, blended
+            if (threadIdx.x < 3) {
+                if (stats) atomicAdd(&stats[3 * view + threadIdx.x], s_stats[threadIdx.x]);
+                tile_out(tile_arg...)[3 * (size_t)blockIdx.x + threadIdx.x] =
+                    threadIdx.x ? s_stats[threadIdx.x] : (unsigned long long)total;
+            }
+        } else {
+            if (threadIdx.x < 3) atomicAdd(&stats[3 * view + threadIdx.x], s_stats[threadIdx.x]);
+        }
     }
 }
 
@@ -944,24 +974,25 @@ k_blend_bwd_seg(int W, int H, int tiles_per_view, const float4 *__restrict__ rec
     }
 }
 
-template <bool STATS, bool CKPT>
+// tile: none, or one unsigned long long * (per-tile statistics)
+template <bool STATS, bool CKPT, typename... TileOut>
 static void launch_fwd(int grid, cudaStream_t stream, int W, int H, int T1, const float *rec, const float *bg,
                        const uint8_t *cl, const uint32_t *ranges, const uint32_t *ids, float *image, float *final_T,
-                       uint32_t *n_contrib, int64_t *stats, const SegWs &seg) {
+                       uint32_t *n_contrib, int64_t *stats, const SegWs &seg, TileOut... tile) {
     if (g_gs_debug_flags & GS_DEBUG_FWD_HALFWARP)
-        k_blend_fwd<STATS, CKPT><<<grid, BL_THREADS, 0, stream>>>(
+        k_blend_fwd<STATS, CKPT, TileOut...><<<grid, BL_THREADS, 0, stream>>>(
             W, H, T1, reinterpret_cast<const float4 *>(rec), bg, cl, reinterpret_cast<const uint2 *>(ranges), ids, image,
-            final_T, n_contrib, reinterpret_cast<unsigned long long *>(stats), seg);
+            final_T, n_contrib, reinterpret_cast<unsigned long long *>(stats), seg, tile...);
     else
-        k_blend_fwd2<STATS, CKPT><<<grid, F2_THREADS, 0, stream>>>(
+        k_blend_fwd2<STATS, CKPT, TileOut...><<<grid, F2_THREADS, 0, stream>>>(
             W, H, T1, reinterpret_cast<const float4 *>(rec), bg, cl, reinterpret_cast<const uint2 *>(ranges), ids, image,
-            final_T, n_contrib, reinterpret_cast<unsigned long long *>(stats), seg);
+            final_T, n_contrib, reinterpret_cast<unsigned long long *>(stats), seg, tile...);
 }
 
 int gs_launch_blend_forward(int num_views, int64_t R, int H, int W, const float *rec, const float *bg,
                             const uint8_t *compute_locally, const uint32_t *ranges, const uint32_t *ids_sorted,
-                            float *image, float *final_T, uint32_t *n_contrib, int64_t *stats, void *seg_ws,
-                            size_t seg_ws_bytes, cudaStream_t stream) {
+                            float *image, float *final_T, uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats,
+                            void *seg_ws, size_t seg_ws_bytes, cudaStream_t stream) {
     const int gx = (W + GS_BLOCK_X - 1) / GS_BLOCK_X, gy = (H + GS_BLOCK_Y - 1) / GS_BLOCK_Y;
     const int T1 = gx * gy;
     SegWs seg = {nullptr, nullptr, nullptr, nullptr};
@@ -978,14 +1009,20 @@ int gs_launch_blend_forward(int num_views, int64_t R, int H, int W, const float 
     if (stats) GS_CUDA_TRY(cudaMemsetAsync(stats, 0, 3 * sizeof(int64_t) * (size_t)num_views, stream));
     GsStageTimer timer(GS_STAGE_BLEND_FWD, stream);
     const int grid = T1 * num_views;
-    if (stats && seg_ws)
+    unsigned long long *ts = reinterpret_cast<unsigned long long *>(tile_stats);
+    if (stats && seg_ws && !tile_stats)
         launch_fwd<true, true>(grid, stream, W, H, T1, rec, bg, compute_locally, ranges, ids_sorted, image, final_T, n_contrib, stats, seg);
-    else if (stats)
+    else if (stats && !tile_stats)
         launch_fwd<true, false>(grid, stream, W, H, T1, rec, bg, compute_locally, ranges, ids_sorted, image, final_T, n_contrib, stats, seg);
-    else if (seg_ws)
+    else if (seg_ws && !tile_stats)
         launch_fwd<false, true>(grid, stream, W, H, T1, rec, bg, compute_locally, ranges, ids_sorted, image, final_T, n_contrib, stats, seg);
-    else
+    else if (!tile_stats)
         launch_fwd<false, false>(grid, stream, W, H, T1, rec, bg, compute_locally, ranges, ids_sorted, image, final_T, n_contrib, stats, seg);
+    // per-tile statistics: every CTA writes its own row, local or not (no memset)
+    else if (seg_ws)
+        launch_fwd<true, true>(grid, stream, W, H, T1, rec, bg, compute_locally, ranges, ids_sorted, image, final_T, n_contrib, stats, seg, ts);
+    else
+        launch_fwd<true, false>(grid, stream, W, H, T1, rec, bg, compute_locally, ranges, ids_sorted, image, final_T, n_contrib, stats, seg, ts);
     GS_LAUNCH_CHECK();
     return GS_OK;
 }

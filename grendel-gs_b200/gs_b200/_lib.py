@@ -69,6 +69,10 @@ SIGNATURES = {
     "gs_render_count_read": (_i, [_vp, C.POINTER(_i64), _vp]),
     "gs_render_forward_batched": (_i, [_i, _vp, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                        _sz, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "gs_render_forward_ts": (_i, [_i, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
+                                  _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "gs_render_forward_batched_ts": (_i, [_i, _vp, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                          _vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "gs_render_backward_batched": (_i, [_i, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp,
                                         _vp, _vp]),
     "gs_loss_temp_bytes_batched": (_sz, [_i, _vp, _i]),
@@ -167,16 +171,36 @@ def debug_set(flags):
     return query("gs_debug_set", int(flags))
 
 
+PROFILE_ON = False   # the state profile_enable() last set
+_PROFILE_CARRY = {}  # stage times profile_carry() handed back to the next profile_read()
+
+
 def profile_enable(on=True):
+    global PROFILE_ON
     call("gs_profile_enable", 1 if on else 0)
+    PROFILE_ON = bool(on)
+
+
+def _add_stages(out, stages):
+    for name, (ms, n) in stages.items():
+        ms0, n0 = out.get(name, (0.0, 0))
+        out[name] = (ms0 + ms, n0 + n)
 
 
 def profile_read():
     """-> {stage name: (total ms, launches)} for every stage that recorded launches; resets the counters."""
     out = {}
+    _add_stages(out, _PROFILE_CARRY)
+    _PROFILE_CARRY.clear()
     for st in range(STAGE_NUM):
         ms, n = C.c_double(0.0), C.c_int64(0)
         call("gs_profile_read", st, C.byref(ms), C.byref(n))
         if n.value:
-            out[load().gs_profile_stage_name(st).decode()] = (ms.value, n.value)
+            _add_stages(out, {load().gs_profile_stage_name(st).decode(): (ms.value, n.value)})
     return out
+
+
+def profile_carry(stages):
+    """Hand stage times ({name: (ms, launches)}, as profile_read returns them) back to the next profile_read(): a caller
+    that reads the profiler while someone else has it on leaves that reader's totals whole."""
+    _add_stages(_PROFILE_CARRY, stages)

@@ -5,12 +5,13 @@
   render_gaussians      /root/reference/gaussian_renderer/__init__.py:1271-1282
   get_local2j_ids_bool  /root/reference/gaussian_renderer/workload_division.py:721-744
 """
+import contextlib
 import ctypes as C
 import os
 
 import torch
 
-from . import _lib
+from . import _lib, statlog
 
 BLOCK_X, BLOCK_Y, ONE_DIM_BLOCK_SIZE = 16, 16, 256
 LAST_R_TOTAL = 0  # instances binned by the most recent render_gaussians calls (reset by the caller)
@@ -122,6 +123,53 @@ def _stored_degree(K, sh_degree, what):
     return D
 
 
+# The reference's --zhx_time keys (analyze_statistic.py:1972-1991) per operator call, and the gs_profile stage
+# (gs_profile_stage_name) each one is read from.  None: the fork times the three statistics sums (81-83) as stages of their
+# own; here they are fused into the blend forward (stage 70), so their keys read 0.  Stage 24 is written with the time of
+# k_count_tiles, which covers the reference's 21-24; 24 is the column analyze_statistic.py sums.
+REFERENCE_STAGE_KEYS = {
+    "preprocess forward": (("10 preprocess time", "10 preprocess"),),
+    "render forward": (("24 updateDistributedStatLocally.updateTileTouched time", "21-24 count local tiles"),
+                       ("30 InclusiveSum time", "30 InclusiveSum"), ("40 duplicateWithKeys time", "40 duplicateWithKeys"),
+                       ("50 SortPairs time", "50 SortPairs"), ("60 identifyTileRanges time", "60 identifyTileRanges"),
+                       ("70 render time", "70 render"), ("81 sum_n_render time", None),
+                       ("82 sum_n_consider time", None), ("83 sum_n_contrib time", None)),
+    "render backward": (("b10 render time", "b10 render"),),
+    "preprocess backward": (("b20 preprocess time", "b20 preprocess"),),
+}
+
+
+def reference_stage_times(call, stages):
+    """[(reference key, ms)] of one operator call (a REFERENCE_STAGE_KEYS key) from _lib.profile_read() output; a stage
+    without launches (no instances: nothing to sort) reads 0."""
+    return [(key, 0.0 if st is None else float(stages.get(st, (0.0, 0))[0])) for key, st in REFERENCE_STAGE_KEYS[call]]
+
+
+@contextlib.contextmanager
+def _gpu_time(log, call):
+    """--zhx_time around one operator call's launches: on a logging call (log.time) the profiler is switched on for the
+    block, its stages are read back (a host sync, on logging iterations only), the profiler is put back as it was -- any
+    times it held are handed back to its own reader -- and the call's block is appended to the gpu_time log.  Otherwise
+    nothing at all happens."""
+    if log is None or not log.time:
+        yield
+        return
+    was_on = _lib.PROFILE_ON
+    held = _lib.profile_read() if was_on else {}
+    _lib.profile_enable(True)
+    stages = {}
+    try:
+        yield
+        stages = _lib.profile_read()
+    finally:
+        _lib.profile_enable(was_on)
+        if was_on:
+            _lib.profile_carry(held)
+            _lib.profile_carry(stages)
+    statlog.append(log.path("gpu_time"), statlog.gpu_time_text(
+        log.iteration, f"rk={log.global_rank}, ws={log.world_size}, {call}", reference_stage_times(call, stages)))
+
+
 def _grad_or_zeros(g, shape, dev):
     """An incoming gradient as contiguous fp32, or zeros where autograd passes None for an unused output."""
     return torch.zeros(shape, dtype=torch.float32, device=dev) if g is None else _f32c(g, "grad")
@@ -129,7 +177,7 @@ def _grad_or_zeros(g, shape, dev):
 
 class _PreprocessGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, scales, rotations, shs, opacities, rs):
+    def forward(ctx, means3D, scales, rotations, shs, opacities, rs, log):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         means3D, scales, rotations = _f32c(means3D, "means3D"), _f32c(scales, "scales"), _f32c(rotations, "rotations")
         shs, opacities = _f32c(shs, "shs"), _f32c(opacities, "opacities")
@@ -143,12 +191,13 @@ class _PreprocessGaussians(torch.autograd.Function):
         dev = means3D.device
         vm, pm, cp = _f32c(rs.viewmatrix, "viewmatrix"), _f32c(rs.projmatrix, "projmatrix"), _f32c(rs.campos, "campos")
         means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((P,), dev)
-        _lib.call("gs_preprocess_forward_sh", P, int(rs.sh_degree), max_deg, means3D.data_ptr(), scales.data_ptr(),
-                  float(rs.scale_modifier), rotations.data_ptr(), opacities.data_ptr(), shs.data_ptr(), vm.data_ptr(),
-                  pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
-                  float(rs.tanfovy), means2D.data_ptr(), depths.data_ptr(), radii.data_ptr(), conic_opacity.data_ptr(),
-                  rgb.data_ptr(), clamped.data_ptr(), _stream())
-        ctx.rs, ctx.max_deg = rs, max_deg
+        with _gpu_time(log, "preprocess forward"):
+            _lib.call("gs_preprocess_forward_sh", P, int(rs.sh_degree), max_deg, means3D.data_ptr(), scales.data_ptr(),
+                      float(rs.scale_modifier), rotations.data_ptr(), opacities.data_ptr(), shs.data_ptr(), vm.data_ptr(),
+                      pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
+                      float(rs.tanfovy), means2D.data_ptr(), depths.data_ptr(), radii.data_ptr(),
+                      conic_opacity.data_ptr(), rgb.data_ptr(), clamped.data_ptr(), _stream())
+        ctx.rs, ctx.max_deg, ctx.log = rs, max_deg, log
         ctx.cam = (vm, pm, cp)
         ctx.save_for_backward(means3D, scales, rotations, shs, radii, clamped)
         ctx.mark_non_differentiable(radii, depths)
@@ -168,19 +217,23 @@ class _PreprocessGaussians(torch.autograd.Function):
         d_rot = torch.empty((P, 4), dtype=torch.float32, device=dev)
         d_opac = torch.empty((P, 1), dtype=torch.float32, device=dev)
         d_shs = torch.empty(tuple(shs.shape), dtype=torch.float32, device=dev)
-        _lib.call("gs_preprocess_backward_sh", P, int(rs.sh_degree), ctx.max_deg, means3D.data_ptr(),
-                  scales.data_ptr(), float(rs.scale_modifier), rotations.data_ptr(), shs.data_ptr(), vm.data_ptr(),
-                  pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
-                  float(rs.tanfovy), radii.data_ptr(), clamped.data_ptr(), g_means2D.data_ptr(),
-                  g_conic_opacity.data_ptr(), g_rgb.data_ptr(), d_means3D.data_ptr(), d_scales.data_ptr(),
-                  d_rot.data_ptr(), d_opac.data_ptr(), d_shs.data_ptr(), _stream())
-        return d_means3D, d_scales, d_rot, d_shs, d_opac, None
+        with _gpu_time(ctx.log, "preprocess backward"):
+            _lib.call("gs_preprocess_backward_sh", P, int(rs.sh_degree), ctx.max_deg, means3D.data_ptr(),
+                      scales.data_ptr(), float(rs.scale_modifier), rotations.data_ptr(), shs.data_ptr(), vm.data_ptr(),
+                      pm.data_ptr(), cp.data_ptr(), int(rs.image_width), int(rs.image_height), float(rs.tanfovx),
+                      float(rs.tanfovy), radii.data_ptr(), clamped.data_ptr(), g_means2D.data_ptr(),
+                      g_conic_opacity.data_ptr(), g_rgb.data_ptr(), d_means3D.data_ptr(), d_scales.data_ptr(),
+                      d_rot.data_ptr(), d_opac.data_ptr(), d_shs.data_ptr(), _stream())
+        return d_means3D, d_scales, d_rot, d_shs, d_opac, None, None
 
 
 def preprocess_gaussians(means3D, scales, rotations, shs, opacities, raster_settings, cuda_args=None):
     """-> (means2D (P,2) pixels, rgb (P,3), conic_opacity (P,4), radii (P) int32, depths (P)).
-    shs (P,K,3): the K = (D+1)^2 coefficients of a model stored at degree D = 0..3; raster_settings.sh_degree <= D."""
-    return _PreprocessGaussians.apply(means3D, scales, rotations, shs, opacities, raster_settings)
+    shs (P,K,3): the K = (D+1)^2 coefficients of a model stored at degree D = 0..3; raster_settings.sh_degree <= D.
+    cuda_args: the reference's dict; with zhx_time "True" on a logging iteration (statlog.request) this call and its
+    backward append stages 10 and b20 to the gpu_time log."""
+    return _PreprocessGaussians.apply(means3D, scales, rotations, shs, opacities, raster_settings,
+                                      statlog.request(cuda_args))
 
 
 class _PreprocessGaussiansRaw(torch.autograd.Function):
@@ -302,7 +355,7 @@ def _grad_block(P, dev):
 
 class _RenderGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, rs, collector):
+    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, rs, collector, want_ts, log):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         means2D, conic_opacity, rgb = _f32c(means2D, "means2D"), _f32c(conic_opacity, "conic_opacity"), _f32c(rgb, "rgb")
         depths = _f32c(depths, "depths")
@@ -336,31 +389,40 @@ class _RenderGaussians(torch.autograd.Function):
         final_T = torch.empty((H, W), dtype=torch.float32, device=dev)
         n_contrib = torch.empty((H, W), dtype=torch.int32, device=dev)
         stats = torch.empty((3,), dtype=torch.int64, device=dev)
+        log_tiles = log is not None and log.debug
+        ts = torch.empty((ty, tx, 3), dtype=torch.int64, device=dev) if want_ts or log_tiles else None
         needs_grad = means2D.requires_grad or conic_opacity.requires_grad or rgb.requires_grad
-        R = C.c_int64(0)
-        ticket = C.c_void_p()
-        _lib.call("gs_render_count_launch", 1, None, P, H, W, means2D.data_ptr(), conic_opacity.data_ptr(), rgb.data_ptr(),
-                  depths.data_ptr(), radii.data_ptr(), cl.data_ptr(), order.data_ptr(), offsets.data_ptr(),
-                  rec.data_ptr(), temp.data_ptr(), tb, C.byref(ticket), s)
-        key = (1, H, W, needs_grad)          # not P: the splat count of a strip varies from step to step, R follows it smoothly
-        pre = _instance_buffers_before_sync(key, T, dev, needs_grad)    # host work while the count / sort / scan run
-        _lib.call("gs_render_count_read", ticket, C.byref(R), s)   # the operator's one host sync
-        R = int(R.value)
-        global LAST_R_TOTAL
-        LAST_R_TOTAL += R
-        ib = _instance_buffers_after_sync(key, pre, R, T, dev, needs_grad)
-        seg = ib.seg if R > 0 else None
-        _lib.call("gs_render_forward", P, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
-                  order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
-                  ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(),
-                  image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(seg),
-                  ib.segb if seg is not None else 0, s)
-        ev1.record()
+        with _gpu_time(log, "render forward"):   # the count, the sort and the blend of this call (stages 24-70)
+            R = C.c_int64(0)
+            ticket = C.c_void_p()
+            _lib.call("gs_render_count_launch", 1, None, P, H, W, means2D.data_ptr(), conic_opacity.data_ptr(), rgb.data_ptr(),
+                      depths.data_ptr(), radii.data_ptr(), cl.data_ptr(), order.data_ptr(), offsets.data_ptr(),
+                      rec.data_ptr(), temp.data_ptr(), tb, C.byref(ticket), s)
+            key = (1, H, W, needs_grad)          # not P: the splat count of a strip varies from step to step, R follows it smoothly
+            pre = _instance_buffers_before_sync(key, T, dev, needs_grad)    # host work while the count / sort / scan run
+            _lib.call("gs_render_count_read", ticket, C.byref(R), s)   # the operator's one host sync
+            R = int(R.value)
+            global LAST_R_TOTAL
+            LAST_R_TOTAL += R
+            ib = _instance_buffers_after_sync(key, pre, R, T, dev, needs_grad)
+            seg = ib.seg if R > 0 else None
+            _lib.call("gs_render_forward_ts", P, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
+                      order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
+                      ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(),
+                      image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts),
+                      _lib.ptr(seg), ib.segb if seg is not None else 0, s)
+            ev1.record()
+        if log_tiles:
+            statlog.append(log.path("n_contrib"), statlog.n_contrib_text(
+                log.iteration, log.local_rank, log.world_size, H, W, cl.cpu(), ranges.cpu(), ts.cpu()))
         _timed(collector, "forward_render_time", ev0, ev1)
         ids_sorted = ib.ids[1]    # a view: the (tile, id) scratch stays alive until the backward has run (16 B / instance)
-        ctx.rs, ctx.R, ctx.P, ctx.collector, ctx.seg = rs, R, P, collector, seg
+        ctx.rs, ctx.R, ctx.P, ctx.collector, ctx.seg, ctx.log = rs, R, P, collector, seg, log
         ctx.save_for_backward(rec, bg, cl, ranges, ids_sorted, final_T, n_contrib)
         n_render, n_consider, n_contrib_sum = stats[0], stats[1], stats[2]
+        if want_ts:
+            ctx.mark_non_differentiable(n_render, n_consider, n_contrib_sum, ts)
+            return image, n_render, n_consider, n_contrib_sum, ts
         ctx.mark_non_differentiable(n_render, n_consider, n_contrib_sum)
         return image, n_render, n_consider, n_contrib_sum
 
@@ -375,19 +437,26 @@ class _RenderGaussians(torch.autograd.Function):
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
         seg = ctx.seg
-        _lib.call("gs_render_backward", P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(), ranges.data_ptr(),
-                  ids_sorted.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), g_image.data_ptr(),
-                  _lib.ptr(seg), 0 if seg is None else seg.numel(),
-                  d_means2D.data_ptr(), d_conic.data_ptr(), d_rgb.data_ptr(), _stream())
+        with _gpu_time(ctx.log, "render backward"):
+            _lib.call("gs_render_backward", P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(), ranges.data_ptr(),
+                      ids_sorted.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), g_image.data_ptr(),
+                      _lib.ptr(seg), 0 if seg is None else seg.numel(),
+                      d_means2D.data_ptr(), d_conic.data_ptr(), d_rgb.data_ptr(), _stream())
         ctx.seg = None
         ev1.record()
         _timed(ctx.collector, "backward_render_time", ev0, ev1)
-        return d_means2D, d_conic, d_rgb, None, None, None, None, None
+        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None, None
 
 
 def render_gaussians(means2D, conic_opacity, rgb, depths, radii, compute_locally, raster_settings, cuda_args=None,
-                     extended_compute_locally=None):
-    """-> (image (3,H,W) with non-local tiles exactly 0, n_render, n_consider, n_contrib).
+                     extended_compute_locally=None, *, tile_stats=False):
+    """-> (image (3,H,W) with non-local tiles exactly 0, n_render, n_consider, n_contrib), and with tile_stats=True also
+    (TILE_Y, TILE_X, 3) int64: per tile the list length, the entries walked and the entries blended summed over the tile's
+    in-image pixels (gs_render_forward_ts; non-local tiles read 0).
+
+    cuda_args: the reference's dict.  On a logging iteration (statlog.request) zhx_time "True" appends stages 24-83 of
+    this call and b10 of its backward to the gpu_time log, and zhx_debug "True" appends this call's per-tile lines and
+    summary to the n_contrib log.
 
     extended_compute_locally: the live path passes None (workload_division.py:802-803); the legacy render()
     (gaussian_renderer/__init__.py:458-507) passes the local tile region dilated by one tile
@@ -404,7 +473,8 @@ def render_gaussians(means2D, conic_opacity, rgb, depths, radii, compute_locally
     collector = None
     if isinstance(cuda_args, dict):
         collector = cuda_args.setdefault("stats_collector", {})
-    return _RenderGaussians.apply(means2D, conic_opacity, rgb, depths, radii, compute_locally, raster_settings, collector)
+    return _RenderGaussians.apply(means2D, conic_opacity, rgb, depths, radii, compute_locally, raster_settings, collector,
+                                  bool(tile_stats), statlog.request(cuda_args))
 
 
 MAX_VIEWS = 64   # GS_MAX_VIEWS
@@ -419,7 +489,7 @@ class _RenderGaussiansBatched(torch.autograd.Function):
     concatenated (camera k = rows [view_start[k], view_start[k+1])), masks (B,T), images (B,3,H,W)."""
 
     @staticmethod
-    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, view_start, rs, collector):
+    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, view_start, rs, collector, want_ts):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         means2D, conic_opacity, rgb = _f32c(means2D, "means2D"), _f32c(conic_opacity, "conic_opacity"), _f32c(rgb, "rgb")
         depths = _f32c(depths, "depths")
@@ -459,6 +529,7 @@ class _RenderGaussiansBatched(torch.autograd.Function):
         final_T = torch.empty((B, H, W), dtype=torch.float32, device=dev)
         n_contrib = torch.empty((B, H, W), dtype=torch.int32, device=dev)
         stats = torch.empty((B, 3), dtype=torch.int64, device=dev)
+        ts = torch.empty((B, ty, tx, 3), dtype=torch.int64, device=dev) if want_ts else None
         needs_grad = means2D.requires_grad or conic_opacity.requires_grad or rgb.requires_grad
         R = C.c_int64(0)
         ticket = C.c_void_p()
@@ -473,21 +544,24 @@ class _RenderGaussiansBatched(torch.autograd.Function):
         LAST_R_TOTAL += R
         ib = _instance_buffers_after_sync(key, pre, R, B * T, dev, needs_grad)
         seg = ib.seg if R > 0 else None
-        _lib.call("gs_render_forward_batched", B, vs, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
+        _lib.call("gs_render_forward_batched_ts", B, vs, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
                   order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
                   ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(),
-                  image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(seg),
-                  ib.segb if seg is not None else 0, s)
+                  image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts),
+                  _lib.ptr(seg), ib.segb if seg is not None else 0, s)
         ev1.record()
         _timed(collector, "forward_render_time", ev0, ev1)
         ids_sorted = ib.ids[1]    # a view: the (tile, id) scratch stays alive until the backward has run (16 B / instance)
         ctx.rs, ctx.R, ctx.P, ctx.B, ctx.collector, ctx.seg = rs, R, P, B, collector, seg
         ctx.save_for_backward(rec, bg, cl, ranges, ids_sorted, final_T, n_contrib)
+        if want_ts:
+            ctx.mark_non_differentiable(stats, ts)
+            return image, stats, ts
         ctx.mark_non_differentiable(stats)
         return image, stats
 
     @staticmethod
-    def backward(ctx, g_image, _g_stats):
+    def backward(ctx, g_image, *_unused):
         rec, bg, cl, ranges, ids_sorted, final_T, n_contrib = ctx.saved_tensors
         rs, R, P, B = ctx.rs, ctx.R, ctx.P, ctx.B
         H, W = int(rs.image_height), int(rs.image_width)
@@ -504,21 +578,23 @@ class _RenderGaussiansBatched(torch.autograd.Function):
         ctx.seg = None
         ev1.record()
         _timed(ctx.collector, "backward_render_time", ev0, ev1)
-        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None
+        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None, None
 
 
 def render_gaussians_batched(means2D, conic_opacity, rgb, depths, radii, compute_locally, view_start, raster_settings,
-                             cuda_args=None):
+                             cuda_args=None, *, tile_stats=False):
     """All B cameras of a batch in one pass.  means2D (N,2), conic_opacity (N,4), rgb (N,3), depths (N), radii (N):
     the splats of the B cameras concatenated, camera k = rows [view_start[k], view_start[k+1]) (len(view_start) = B+1);
     compute_locally (B, TILE_Y*TILE_X) (None = everything local); the cameras share the image size and background of
     `raster_settings` (their view / projection matrices were consumed by the preprocess).
-    -> (images (B,3,H,W) with non-local tiles exactly 0, stats (B,3) int64 = n_render / n_consider / n_contrib)."""
+    -> (images (B,3,H,W) with non-local tiles exactly 0, stats (B,3) int64 = n_render / n_consider / n_contrib), and
+    with tile_stats=True also (B, TILE_Y, TILE_X, 3) int64: slice k is render_gaussians(..., tile_stats=True)'s for
+    camera k."""
     collector = None
     if isinstance(cuda_args, dict):
         collector = cuda_args.setdefault("stats_collector", {})
     return _RenderGaussiansBatched.apply(means2D, conic_opacity, rgb, depths, radii, compute_locally,
-                                         [int(v) for v in view_start], raster_settings, collector)
+                                         [int(v) for v in view_start], raster_settings, collector, bool(tile_stats))
 
 
 class _FusedL1SSIMBatched(torch.autograd.Function):

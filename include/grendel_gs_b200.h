@@ -280,6 +280,30 @@ GS_API int gs_render_forward_batched(int num_views, const int32_t *view_start_ho
                                      size_t sort_temp_bytes, uint32_t *ranges, float *image, float *final_T,
                                      uint32_t *n_contrib, int64_t *stats, void *seg_ws, size_t seg_ws_bytes,
                                      void *stream);
+
+/* gs_render_forward / gs_render_forward_batched with per-tile blend statistics (the per-tile lines of the reference's
+ * --zhx_debug log, n_contrib_ws=W_rk=R.log, analyze_statistic.py:843-962).  tile_stats: (num_views*T, 3) int64, or NULL
+ * (then these calls are gs_render_forward / _batched exactly); 8-byte aligned.  Row v*T + t holds, for tile t of view v,
+ *   [0] the length of the tile's list, [1] sum over the tile's in-image pixels of the entries walked,
+ *   [2] sum over the same pixels of the entries blended.
+ * Non-local tiles and empty lists read 0: every row is written, no memset is needed.  Columns 1 and 2 summed over a
+ * view's tiles equal stats[1] and stats[2]; column 0 times the tile's in-image pixel count sums to stats[0].  stats may be
+ * NULL when tile_stats is not. */
+GS_API int gs_render_forward_ts(int P, int64_t R, int image_height, int image_width, const float *means2D,
+                                const int32_t *radii, const uint8_t *compute_locally, const uint32_t *order,
+                                const uint32_t *offsets, const float *rec, const float *bg, uint32_t *tiles_unsorted,
+                                uint32_t *ids_unsorted, uint32_t *tiles_sorted, uint32_t *ids_sorted, void *sort_temp,
+                                size_t sort_temp_bytes, uint32_t *ranges, float *image, float *final_T,
+                                uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats, void *seg_ws,
+                                size_t seg_ws_bytes, void *stream);
+GS_API int gs_render_forward_batched_ts(int num_views, const int32_t *view_start_host, int64_t R, int image_height,
+                                        int image_width, const float *means2D, const int32_t *radii,
+                                        const uint8_t *compute_locally, const uint32_t *order, const uint32_t *offsets,
+                                        const float *rec, const float *bg, uint32_t *tiles_unsorted,
+                                        uint32_t *ids_unsorted, uint32_t *tiles_sorted, uint32_t *ids_sorted,
+                                        void *sort_temp, size_t sort_temp_bytes, uint32_t *ranges, float *image,
+                                        float *final_T, uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats,
+                                        void *seg_ws, size_t seg_ws_bytes, void *stream);
 GS_API int gs_render_backward_batched(int num_views, int P, int64_t R, int image_height, int image_width,
                                       const float *rec, const float *bg, const uint8_t *compute_locally,
                                       const uint32_t *ranges, const uint32_t *ids_sorted, const float *final_T,
