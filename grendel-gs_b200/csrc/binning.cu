@@ -118,11 +118,15 @@ struct TouchedInDepthOrder {
 };
 
 // Stage 40: one (tile, splat id) pair per (splat, local tile), emitted in DEPTH order of the splats.
+// DET (deterministic render): the sort's payload is the instance's own unsorted slot u (its `off`), written to `slots`,
+// and the splat id goes to `ids` beside it; the same stable key sort then yields sorted_u, from which k_gather_ids forms
+// the sorted ids.  The splat at depth position d owns the unsorted slots [offsets[d-1], offsets[d]).
+template <bool DET>
 __global__ void __launch_bounds__(BIN_THREADS)
 k_duplicate(int P, int W, int H, const float *__restrict__ means2D, const int32_t *__restrict__ radii,
             const uint8_t *__restrict__ compute_locally, const uint32_t *__restrict__ order,
             const uint32_t *__restrict__ offsets, uint32_t *__restrict__ tile_keys, uint32_t *__restrict__ ids,
-            const GsViews views) {
+            const GsViews views, uint32_t *__restrict__ slots) {
     const int s = blockIdx.x * BIN_THREADS + threadIdx.x;
     if (s >= P) return;
     uint32_t off = (s == 0) ? 0u : offsets[s - 1];
@@ -139,8 +143,17 @@ k_duplicate(int P, int W, int H, const float *__restrict__ means2D, const int32_
             if (!compute_locally[t]) continue;
             tile_keys[off] = (uint32_t)t;
             ids[off] = i;
+            if (DET) slots[off] = off;
             off++;
         }
+}
+
+// Deterministic render: ids_sorted[r] = ids_unsorted[sorted_u[r]] -- the list the default sort writes, entry for entry.
+__global__ void __launch_bounds__(BIN_THREADS)
+k_gather_ids(int64_t R, const uint32_t *__restrict__ sorted_u, const uint32_t *__restrict__ ids_unsorted,
+             uint32_t *__restrict__ ids_sorted) {
+    const int64_t r = (int64_t)blockIdx.x * BIN_THREADS + threadIdx.x;
+    if (r < R) ids_sorted[r] = __ldg(ids_unsorted + __ldg(sorted_u + r));
 }
 
 // Stage 60: [start,end) of every tile in the sorted list.  One thread per TILE finds its two boundaries by binary search
@@ -359,15 +372,15 @@ int gs_launch_blend_forward(int num_views, int64_t R, int H, int W, const float 
                             float *image, float *final_T, uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats,
                             void *seg_ws, size_t seg_ws_bytes, cudaStream_t stream);
 
-extern "C" int gs_render_forward_batched_ts(int num_views, const int32_t *view_start, int64_t R, int image_height,
-                                            int image_width, const float *means2D, const int32_t *radii,
-                                            const uint8_t *compute_locally, const uint32_t *order, const uint32_t *offsets,
-                                            const float *rec, const float *bg, uint32_t *tiles_unsorted,
-                                            uint32_t *ids_unsorted, uint32_t *tiles_sorted, uint32_t *ids_sorted,
-                                            void *sort_temp, size_t sort_temp_bytes, uint32_t *ranges, float *image,
-                                            float *final_T, uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats,
-                                            void *seg_ws, size_t seg_ws_bytes, void *stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
+// sorted_u: NULL = the default forward; otherwise the deterministic one (k_duplicate<true> + k_gather_ids), which also
+// leaves sorted_u (R) for gs_render_backward_det
+static int render_forward_impl(int num_views, const int32_t *view_start, int64_t R, int image_height, int image_width,
+                               const float *means2D, const int32_t *radii, const uint8_t *compute_locally,
+                               const uint32_t *order, const uint32_t *offsets, const float *rec, const float *bg,
+                               uint32_t *tiles_unsorted, uint32_t *ids_unsorted, uint32_t *tiles_sorted,
+                               uint32_t *ids_sorted, uint32_t *sorted_u, void *sort_temp, size_t sort_temp_bytes,
+                               uint32_t *ranges, float *image, float *final_T, uint32_t *n_contrib, int64_t *stats,
+                               int64_t *tile_stats, void *seg_ws, size_t seg_ws_bytes, cudaStream_t stream) {
     GS_REQUIRE(R >= 0 && image_height > 0 && image_width > 0, "sizes");
     GS_REQUIRE(R < (1ll << 31), "more than 2^31 splat-tile instances");
     GS_REQUIRE(compute_locally && bg && ranges && image && final_T && n_contrib, "null pointer");
@@ -390,17 +403,36 @@ extern "C" int gs_render_forward_batched_ts(int num_views, const int32_t *view_s
             gs_set_error("gs_render_forward: sort temp too small");
             return GS_ENOMEM;
         }
-        {
-            GsStageTimer timer(GS_STAGE_DUPLICATE, stream);
-            k_duplicate<<<(P + BIN_THREADS - 1) / BIN_THREADS, BIN_THREADS, 0, stream>>>(
-                P, image_width, image_height, means2D, radii, compute_locally, order, offsets, tiles_unsorted, ids_unsorted,
-                views);
-            GS_LAUNCH_CHECK();
-        }
-        {
-            GsStageTimer timer(GS_STAGE_SORT, stream);  // stable sort on the tile bits only
-            GS_CUDA_TRY(cub::DeviceRadixSort::SortPairs(sort_temp, sort_temp_bytes, tiles_unsorted, tiles_sorted,
-                                                        ids_unsorted, ids_sorted, (int)R, 0, tile_bits(T), stream));
+        if (!sorted_u) {
+            {
+                GsStageTimer timer(GS_STAGE_DUPLICATE, stream);
+                k_duplicate<false><<<(P + BIN_THREADS - 1) / BIN_THREADS, BIN_THREADS, 0, stream>>>(
+                    P, image_width, image_height, means2D, radii, compute_locally, order, offsets, tiles_unsorted,
+                    ids_unsorted, views, nullptr);
+                GS_LAUNCH_CHECK();
+            }
+            {
+                GsStageTimer timer(GS_STAGE_SORT, stream);  // stable sort on the tile bits only
+                GS_CUDA_TRY(cub::DeviceRadixSort::SortPairs(sort_temp, sort_temp_bytes, tiles_unsorted, tiles_sorted,
+                                                            ids_unsorted, ids_sorted, (int)R, 0, tile_bits(T), stream));
+            }
+        } else {
+            // the slot payload is staged in ids_sorted, which the gather overwrites once the sort has consumed it
+            {
+                GsStageTimer timer(GS_STAGE_DUPLICATE, stream);
+                k_duplicate<true><<<(P + BIN_THREADS - 1) / BIN_THREADS, BIN_THREADS, 0, stream>>>(
+                    P, image_width, image_height, means2D, radii, compute_locally, order, offsets, tiles_unsorted,
+                    ids_unsorted, views, ids_sorted);
+                GS_LAUNCH_CHECK();
+            }
+            {
+                GsStageTimer timer(GS_STAGE_SORT, stream);  // the same stable key sort, same input order: same permutation
+                GS_CUDA_TRY(cub::DeviceRadixSort::SortPairs(sort_temp, sort_temp_bytes, tiles_unsorted, tiles_sorted,
+                                                            ids_sorted, sorted_u, (int)R, 0, tile_bits(T), stream));
+                k_gather_ids<<<(unsigned)((R + BIN_THREADS - 1) / BIN_THREADS), BIN_THREADS, 0, stream>>>(
+                    R, sorted_u, ids_unsorted, ids_sorted);
+                GS_LAUNCH_CHECK();
+            }
         }
         {
             GsStageTimer timer(GS_STAGE_RANGES, stream);
@@ -410,6 +442,42 @@ extern "C" int gs_render_forward_batched_ts(int num_views, const int32_t *view_s
     }
     return gs_launch_blend_forward(num_views, R, image_height, image_width, rec, bg, compute_locally, ranges, ids_sorted,
                                    image, final_T, n_contrib, stats, tile_stats, seg_ws, seg_ws_bytes, stream);
+}
+
+extern "C" int gs_render_forward_batched_ts(int num_views, const int32_t *view_start, int64_t R, int image_height,
+                                            int image_width, const float *means2D, const int32_t *radii,
+                                            const uint8_t *compute_locally, const uint32_t *order, const uint32_t *offsets,
+                                            const float *rec, const float *bg, uint32_t *tiles_unsorted,
+                                            uint32_t *ids_unsorted, uint32_t *tiles_sorted, uint32_t *ids_sorted,
+                                            void *sort_temp, size_t sort_temp_bytes, uint32_t *ranges, float *image,
+                                            float *final_T, uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats,
+                                            void *seg_ws, size_t seg_ws_bytes, void *stream) {
+    return render_forward_impl(num_views, view_start, R, image_height, image_width, means2D, radii, compute_locally, order,
+                               offsets, rec, bg, tiles_unsorted, ids_unsorted, tiles_sorted, ids_sorted, nullptr, sort_temp,
+                               sort_temp_bytes, ranges, image, final_T, n_contrib, stats, tile_stats, seg_ws, seg_ws_bytes,
+                               (cudaStream_t)stream);
+}
+
+extern "C" int gs_render_forward_det(int num_views, const int32_t *view_start, int P, int64_t R, int image_height,
+                                     int image_width, const float *means2D, const int32_t *radii,
+                                     const uint8_t *compute_locally, const uint32_t *order, const uint32_t *offsets,
+                                     const float *rec, const float *bg, uint32_t *tiles_unsorted, uint32_t *ids_unsorted,
+                                     uint32_t *tiles_sorted, uint32_t *ids_sorted, uint32_t *sorted_u, void *sort_temp,
+                                     size_t sort_temp_bytes, uint32_t *ranges, float *image, float *final_T,
+                                     uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats, void *seg_ws,
+                                     size_t seg_ws_bytes, void *stream) {
+    const int32_t one_view[2] = {0, P};
+    if (view_start == nullptr) {   // the single-camera form, as gs_render_count_launch
+        GS_REQUIRE(num_views == 1 && P >= 0, "view_start may only be NULL for one view");
+        view_start = one_view;
+    }
+    GS_REQUIRE(R == 0 || (sorted_u != nullptr && ids_unsorted != nullptr && ids_sorted != nullptr), "null pointer");
+    GS_REQUIRE(((uintptr_t)sorted_u & 3) == 0 && ((uintptr_t)ids_unsorted & 3) == 0 && ((uintptr_t)ids_sorted & 3) == 0,
+               "instance arrays must be 4-byte aligned");
+    return render_forward_impl(num_views, view_start, R, image_height, image_width, means2D, radii, compute_locally, order,
+                               offsets, rec, bg, tiles_unsorted, ids_unsorted, tiles_sorted, ids_sorted,
+                               R > 0 ? sorted_u : nullptr, sort_temp, sort_temp_bytes, ranges, image, final_T, n_contrib,
+                               stats, tile_stats, seg_ws, seg_ws_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int gs_render_forward_batched(int num_views, const int32_t *view_start, int64_t R, int image_height,

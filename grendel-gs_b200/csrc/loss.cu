@@ -46,16 +46,25 @@ struct LossViews {
 };
 
 // temp layout: [0,16) two double accumulators per view; then maps (3 maps x 3 channels x rows x W per view)
+// DET (deterministic loss): each CTA writes its two fp64 partials to its own slot of `partials` (CTA (x, y) of view v:
+// slot (v gridDim.y + y) gridDim.x + x; CTAs below the view's strip write zeros) instead of adding them atomically into
+// `sums`; k_loss_finalize_det sums the slots in a fixed order.
+template <bool DET>
 __global__ void __launch_bounds__(LS_THREADS)
 k_loss_fwd(int W, int H, const LossViews lv, const float *__restrict__ image, float *__restrict__ maps,
-           double *__restrict__ sums) {
+           double *__restrict__ sums, double *__restrict__ partials) {
     __shared__ float s_x[LS_IN][LS_IN + 1], s_y[LS_IN][LS_IN + 1];
     __shared__ float s_h[5][LS_IN][LS_TILE + 1];
     __shared__ float s_red[2][LS_THREADS / 32];
     const int view = blockIdx.z;
     const int row0 = lv.row0[view], rows = lv.rows[view], crow0 = lv.crow0[view], crow1 = lv.crow1[view];
     const int tx0 = blockIdx.x * LS_TILE, ty0 = blockIdx.y * LS_TILE;  // strip-local tile origin
-    if (ty0 >= rows) return;  // the grid is sized for the tallest strip of the batch
+    if constexpr (DET) partials += 2 * (((size_t)view * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x);
+    if (ty0 >= rows) {  // the grid is sized for the tallest strip of the batch
+        if constexpr (DET)
+            if (threadIdx.x == 0) { partials[0] = 0.0; partials[1] = 0.0; }
+        return;
+    }
     const size_t HW = (size_t)H * W, SW = (size_t)rows * W;
     const uint8_t *__restrict__ gt = lv.gt[view];
     image += (size_t)view * 3 * HW;
@@ -144,13 +153,27 @@ k_loss_fwd(int W, int H, const LossViews lv, const float *__restrict__ image, fl
     if (threadIdx.x == 0) {
         double a = 0.0, b = 0.0;
         for (int w = 0; w < LS_THREADS / 32; w++) { a += (double)s_red[0][w]; b += (double)s_red[1][w]; }
-        atomicAdd(&sums[0], a); atomicAdd(&sums[1], b);
+        if constexpr (DET) { partials[0] = a; partials[1] = b; }
+        else { atomicAdd(&sums[0], a); atomicAdd(&sums[1], b); }
     }
 }
 
 __global__ void k_loss_finalize(int n, const double *__restrict__ sums, double inv_norm, float *__restrict__ out) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;  // 2 values (Ll1, ssim) per view
     if (k < 2 * n) out[k] = (float)(sums[k] * inv_norm);
+}
+
+// One CTA per view, warp 0 sums the Ll1 partials and warp 1 the ssim partials of the view's `slots` CTA slots: lane l adds
+// slots l, l + 32, ... in index order, then a fixed xor butterfly -- the same order on every run.
+__global__ void __launch_bounds__(64)
+k_loss_finalize_det(int slots, const double *__restrict__ partials, double inv_norm, float *__restrict__ out) {
+    const int view = blockIdx.x, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const double *p = partials + 2 * (size_t)view * slots + w;
+    double s = 0.0;
+    for (int k = lane; k < slots; k += 32) s += p[2 * (size_t)k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) out[2 * view + w] = (float)(s * inv_norm);
 }
 
 __global__ void __launch_bounds__(LS_THREADS)
@@ -263,30 +286,54 @@ static int make_loss_views(int num_views, int H, int W, const int32_t *rows4, co
     return GS_OK;
 }
 
+// deterministic form: per-CTA partial slots behind the maps (which keep their offset, so the backward is unchanged)
+static size_t det_maps_bytes(size_t sum_rows, int W) { return ((size_t)9 * sum_rows * W * sizeof(float) + 255) / 256 * 256; }
+static size_t det_slot_bytes(int num_views, int max_rows, int W) {
+    return 2 * sizeof(double) * (size_t)num_views * (size_t)((W + LS_TILE - 1) / LS_TILE) *
+           (size_t)((max_rows + LS_TILE - 1) / LS_TILE);
+}
+
 static int loss_forward_impl(int num_views, int H, int W, const int32_t *rows4, const float *image, const void *const *gts,
-                             float *out, void *temp, size_t temp_bytes, size_t header, cudaStream_t stream) {
+                             float *out, void *temp, size_t temp_bytes, size_t header, bool det, cudaStream_t stream) {
     GS_REQUIRE(image && out && temp, "null pointer");
     LossViews lv;
     int max_rows = 0;
     size_t sum_rows = 0;
     int rc = make_loss_views(num_views, H, W, rows4, gts, lv, &max_rows, &sum_rows);
     if (rc != GS_OK) return rc;
-    if (temp_bytes < header + (size_t)9 * sum_rows * W * sizeof(float)) {
-        gs_set_error("gs_loss_forward: temp too small");
+    const size_t need = det ? header + det_maps_bytes(sum_rows, W) + det_slot_bytes(num_views, max_rows, W)
+                            : header + (size_t)9 * sum_rows * W * sizeof(float);
+    if (temp_bytes < need) {
+        gs_set_error("gs_loss_forward: temp too small (%zu < %zu)", temp_bytes, need);
         return GS_ENOMEM;
     }
+    if (det) GS_REQUIRE(((uintptr_t)temp & 7) == 0, "temp must be 8-byte aligned");
     rc = ensure_gauss();
     if (rc != GS_OK) return rc;
     double *sums = (double *)temp;
     float *maps = (float *)((char *)temp + header);
+    const double inv_norm = 1.0 / (3.0 * (double)H * (double)W);
+    if (det) {
+        double *partials = (double *)((char *)temp + header + det_maps_bytes(sum_rows, W));
+        GsStageTimer timer(GS_STAGE_LOSS_FWD, stream);
+        const int gy = (max_rows + LS_TILE - 1) / LS_TILE, gxl = (W + LS_TILE - 1) / LS_TILE;
+        if (max_rows > 0) {
+            dim3 grid(gxl, gy, num_views);
+            k_loss_fwd<true><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, nullptr, partials);
+            GS_LAUNCH_CHECK();
+        }
+        k_loss_finalize_det<<<num_views, 64, 0, stream>>>(gxl * gy, partials, inv_norm, out);
+        GS_LAUNCH_CHECK();
+        return GS_OK;
+    }
     GS_CUDA_TRY(cudaMemsetAsync(sums, 0, 2 * sizeof(double) * (size_t)num_views, stream));
     GsStageTimer timer(GS_STAGE_LOSS_FWD, stream);
     if (max_rows > 0) {
         dim3 grid((W + LS_TILE - 1) / LS_TILE, (max_rows + LS_TILE - 1) / LS_TILE, num_views);
-        k_loss_fwd<<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, sums);
+        k_loss_fwd<false><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, sums, nullptr);
         GS_LAUNCH_CHECK();
     }
-    k_loss_finalize<<<1, 2 * GS_MAX_VIEWS, 0, stream>>>(num_views, sums, 1.0 / (3.0 * (double)H * (double)W), out);
+    k_loss_finalize<<<1, 2 * GS_MAX_VIEWS, 0, stream>>>(num_views, sums, inv_norm, out);
     GS_LAUNCH_CHECK();
     return GS_OK;
 }
@@ -332,7 +379,23 @@ extern "C" int gs_loss_forward(int image_height, int image_width, int row0, int 
     const int32_t rows4[4] = {row0, row1, count_row0, count_row1};
     const void *gts[1] = {gt_u8};
     return loss_forward_impl(1, image_height, image_width, rows4, image, gts, out_l1_ssim, temp, temp_bytes, LS_HEADER_1,
-                             (cudaStream_t)stream_);
+                             false, (cudaStream_t)stream_);
+}
+
+extern "C" size_t gs_loss_temp_bytes_det(int rows, int image_width) {
+    const int r = rows > 0 ? rows : 0, w = image_width > 0 ? image_width : 0;
+    return LS_HEADER_1 + det_maps_bytes((size_t)r, w) + det_slot_bytes(1, r, w) + 256;
+}
+
+extern "C" int gs_loss_forward_det(int image_height, int image_width, int row0, int row1, int count_row0, int count_row1,
+                                   const float *image, const uint8_t *gt_u8, float *out_l1_ssim, void *temp,
+                                   size_t temp_bytes, void *stream_) {
+    GS_REQUIRE(row1 > row0, "strip rows");
+    GS_REQUIRE(gt_u8, "null pointer");
+    const int32_t rows4[4] = {row0, row1, count_row0, count_row1};
+    const void *gts[1] = {gt_u8};
+    return loss_forward_impl(1, image_height, image_width, rows4, image, gts, out_l1_ssim, temp, temp_bytes, LS_HEADER_1,
+                             true, (cudaStream_t)stream_);
 }
 
 extern "C" size_t gs_loss_temp_bytes_batched(int num_views, const int32_t *rows4_host, int image_width) {
@@ -348,7 +411,26 @@ extern "C" int gs_loss_forward_batched(int num_views, int image_height, int imag
                                        const float *image, const void *const *gt_u8_ptrs_host, float *out_l1_ssim,
                                        void *temp, size_t temp_bytes, void *stream_) {
     return loss_forward_impl(num_views, image_height, image_width, rows4_host, image, gt_u8_ptrs_host, out_l1_ssim, temp,
-                             temp_bytes, LS_HEADER_B, (cudaStream_t)stream_);
+                             temp_bytes, LS_HEADER_B, false, (cudaStream_t)stream_);
+}
+
+extern "C" size_t gs_loss_temp_bytes_batched_det(int num_views, const int32_t *rows4_host, int image_width) {
+    size_t rows = 0;
+    int max_rows = 0;
+    for (int v = 0; v < num_views && rows4_host; v++) {
+        const int r = rows4_host[4 * v + 1] - rows4_host[4 * v];
+        rows += r > 0 ? (size_t)r : 0;
+        max_rows = r > max_rows ? r : max_rows;
+    }
+    const int w = image_width > 0 ? image_width : 0;
+    return LS_HEADER_B + det_maps_bytes(rows, w) + det_slot_bytes(num_views > 0 ? num_views : 0, max_rows, w) + 256;
+}
+
+extern "C" int gs_loss_forward_batched_det(int num_views, int image_height, int image_width, const int32_t *rows4_host,
+                                           const float *image, const void *const *gt_u8_ptrs_host, float *out_l1_ssim,
+                                           void *temp, size_t temp_bytes, void *stream_) {
+    return loss_forward_impl(num_views, image_height, image_width, rows4_host, image, gt_u8_ptrs_host, out_l1_ssim, temp,
+                             temp_bytes, LS_HEADER_B, true, (cudaStream_t)stream_);
 }
 
 extern "C" int gs_loss_backward(int image_height, int image_width, int row0, int row1, int count_row0, int count_row1,

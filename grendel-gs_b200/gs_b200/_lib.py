@@ -75,6 +75,15 @@ SIGNATURES = {
                                           _vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "gs_render_backward_batched": (_i, [_i, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp,
                                         _vp, _vp]),
+    "gs_render_det_bytes": (_sz, [_i64, _i]),
+    "gs_render_forward_det": (_i, [_i, _vp, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                   _vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "gs_render_backward_det": (_i, [_i, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
+                                    _vp, _sz, _vp, _vp, _vp, _vp]),
+    "gs_loss_temp_bytes_det": (_sz, [_i, _i]),
+    "gs_loss_forward_det": (_i, [_i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "gs_loss_temp_bytes_batched_det": (_sz, [_i, _vp, _i]),
+    "gs_loss_forward_batched_det": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "gs_loss_temp_bytes_batched": (_sz, [_i, _vp, _i]),
     "gs_loss_forward_batched": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "gs_loss_backward_batched": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -291,6 +291,12 @@ def preprocess_gaussians_raw(xyz, features_dc, features_rest, scaling, rotation,
     return _PreprocessGaussiansRaw.apply(xyz, features_dc, features_rest, scaling, rotation, opacity, raster_settings)
 
 
+def deterministic_enabled(deterministic=None):
+    """The operators' `deterministic` argument: None follows torch.use_deterministic_algorithms (PyTorch's switch: an op
+    runs a deterministic implementation or raises), True / False force the choice for one call."""
+    return torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
+
+
 def _tiles(rs):
     return (int(rs.image_height) + BLOCK_Y - 1) // BLOCK_Y, (int(rs.image_width) + BLOCK_X - 1) // BLOCK_X
 
@@ -311,30 +317,40 @@ _R_HINT = {}
 
 
 class _InstanceBuffers:
-    __slots__ = ("cap", "tiles", "ids", "sort_temp", "sb", "seg", "segb")
+    """det: also sorted_u (cap), kept with the rest until the backward has run (the deterministic backward's workspace,
+    _det_workspace, follows the same capacity)."""
+    __slots__ = ("cap", "tiles", "ids", "sort_temp", "sb", "seg", "segb", "sorted_u")
 
-    def __init__(self, cap, num_tiles, dev, needs_grad):
+    def __init__(self, cap, num_tiles, dev, needs_grad, det=False):
         self.cap = _q(cap)
         self.tiles = torch.empty((2, self.cap), dtype=torch.int32, device=dev)
         self.ids = torch.empty((2, self.cap), dtype=torch.int32, device=dev)
         self.sb = _lib.query("gs_render_sort_temp_bytes", self.cap)
         self.sort_temp = torch.empty((self.sb,), dtype=torch.uint8, device=dev)
         self.seg, self.segb = _seg_workspace(self.cap, num_tiles, dev, needs_grad)
+        self.sorted_u = torch.empty((self.cap,), dtype=torch.int32, device=dev) if det else None
 
     def row(self, t, r):
         return t.data_ptr() + 4 * self.cap * r
 
 
-def _instance_buffers_before_sync(key, num_tiles, dev, needs_grad):
+def _det_workspace(ib, Pq, dev):
+    """Instance-gradient rows (36 B per instance), the depth rank and the long-range list (8 B per splat) of
+    gs_render_backward_det, sized
+    from the instance buffers' quantised capacity and the quantised splat count."""
+    return torch.empty((_lib.query("gs_render_det_bytes", ib.cap, Pq),), dtype=torch.uint8, device=dev)
+
+
+def _instance_buffers_before_sync(key, num_tiles, dev, needs_grad, det=False):
     est = _R_HINT.get(key)
-    return None if est is None else _InstanceBuffers(est + est // 12 + 4096, num_tiles, dev, needs_grad)
+    return None if est is None else _InstanceBuffers(est + est // 12 + 4096, num_tiles, dev, needs_grad, det)
 
 
-def _instance_buffers_after_sync(key, pre, R, num_tiles, dev, needs_grad):
+def _instance_buffers_after_sync(key, pre, R, num_tiles, dev, needs_grad, det=False):
     _R_HINT[key] = R
     if pre is not None and R <= pre.cap and (R > 0 or pre.seg is None):
         return pre
-    return _InstanceBuffers(R, num_tiles, dev, needs_grad)
+    return _InstanceBuffers(R, num_tiles, dev, needs_grad, det)
 
 
 def _q(n):
@@ -355,7 +371,7 @@ def _grad_block(P, dev):
 
 class _RenderGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, rs, collector, want_ts, log):
+    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, rs, collector, want_ts, log, det):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         means2D, conic_opacity, rgb = _f32c(means2D, "means2D"), _f32c(conic_opacity, "conic_opacity"), _f32c(rgb, "rgb")
         depths = _f32c(depths, "depths")
@@ -392,25 +408,35 @@ class _RenderGaussians(torch.autograd.Function):
         log_tiles = log is not None and log.debug
         ts = torch.empty((ty, tx, 3), dtype=torch.int64, device=dev) if want_ts or log_tiles else None
         needs_grad = means2D.requires_grad or conic_opacity.requires_grad or rgb.requires_grad
+        det = det and needs_grad    # a forward-only render is the same bits either way
         with _gpu_time(log, "render forward"):   # the count, the sort and the blend of this call (stages 24-70)
             R = C.c_int64(0)
             ticket = C.c_void_p()
             _lib.call("gs_render_count_launch", 1, None, P, H, W, means2D.data_ptr(), conic_opacity.data_ptr(), rgb.data_ptr(),
                       depths.data_ptr(), radii.data_ptr(), cl.data_ptr(), order.data_ptr(), offsets.data_ptr(),
                       rec.data_ptr(), temp.data_ptr(), tb, C.byref(ticket), s)
-            key = (1, H, W, needs_grad)          # not P: the splat count of a strip varies from step to step, R follows it smoothly
-            pre = _instance_buffers_before_sync(key, T, dev, needs_grad)    # host work while the count / sort / scan run
+            # not P: the splat count of a strip varies from step to step, R follows it smoothly
+            key = (1, H, W, needs_grad) if not det else (1, H, W, needs_grad, "det")
+            pre = _instance_buffers_before_sync(key, T, dev, needs_grad, det)    # host work while the count / sort / scan run
             _lib.call("gs_render_count_read", ticket, C.byref(R), s)   # the operator's one host sync
             R = int(R.value)
             global LAST_R_TOTAL
             LAST_R_TOTAL += R
-            ib = _instance_buffers_after_sync(key, pre, R, T, dev, needs_grad)
+            ib = _instance_buffers_after_sync(key, pre, R, T, dev, needs_grad, det)
             seg = ib.seg if R > 0 else None
-            _lib.call("gs_render_forward_ts", P, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
-                      order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
-                      ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(),
-                      image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts),
-                      _lib.ptr(seg), ib.segb if seg is not None else 0, s)
+            if det:
+                _lib.call("gs_render_forward_det", 1, None, P, R, H, W, means2D.data_ptr(), radii.data_ptr(),
+                          cl.data_ptr(), order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(),
+                          ib.row(ib.tiles, 0), ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1),
+                          ib.sorted_u.data_ptr(), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(), image.data_ptr(),
+                          final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts), _lib.ptr(seg),
+                          ib.segb if seg is not None else 0, s)
+            else:
+                _lib.call("gs_render_forward_ts", P, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
+                          order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
+                          ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(),
+                          image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts),
+                          _lib.ptr(seg), ib.segb if seg is not None else 0, s)
             ev1.record()
         if log_tiles:
             statlog.append(log.path("n_contrib"), statlog.n_contrib_text(
@@ -418,6 +444,8 @@ class _RenderGaussians(torch.autograd.Function):
         _timed(collector, "forward_render_time", ev0, ev1)
         ids_sorted = ib.ids[1]    # a view: the (tile, id) scratch stays alive until the backward has run (16 B / instance)
         ctx.rs, ctx.R, ctx.P, ctx.collector, ctx.seg, ctx.log = rs, R, P, collector, seg, log
+        # deterministic backward: the depth order and offsets of the count, the slots of the sort and the row workspace
+        ctx.det = (order, offsets, ib.sorted_u, _det_workspace(ib, Pq, dev)) if det else None
         ctx.save_for_backward(rec, bg, cl, ranges, ids_sorted, final_T, n_contrib)
         n_render, n_consider, n_contrib_sum = stats[0], stats[1], stats[2]
         if want_ts:
@@ -438,21 +466,40 @@ class _RenderGaussians(torch.autograd.Function):
         ev0.record()
         seg = ctx.seg
         with _gpu_time(ctx.log, "render backward"):
-            _lib.call("gs_render_backward", P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(), ranges.data_ptr(),
-                      ids_sorted.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), g_image.data_ptr(),
-                      _lib.ptr(seg), 0 if seg is None else seg.numel(),
-                      d_means2D.data_ptr(), d_conic.data_ptr(), d_rgb.data_ptr(), _stream())
-        ctx.seg = None
+            if ctx.det is not None:
+                _render_backward_det(ctx.det, 1, P, R, H, W, rec, bg, cl, ranges, ids_sorted, final_T, n_contrib,
+                                     g_image, seg, d_means2D, d_conic, d_rgb)
+            else:
+                _lib.call("gs_render_backward", P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(), ranges.data_ptr(),
+                          ids_sorted.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), g_image.data_ptr(),
+                          _lib.ptr(seg), 0 if seg is None else seg.numel(),
+                          d_means2D.data_ptr(), d_conic.data_ptr(), d_rgb.data_ptr(), _stream())
+        ctx.seg = ctx.det = None
         ev1.record()
         _timed(ctx.collector, "backward_render_time", ev0, ev1)
-        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None, None
+        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None, None, None
+
+
+def _render_backward_det(det, B, P, R, H, W, rec, bg, cl, ranges, ids_sorted, final_T, n_contrib, g_image, seg, d_means2D,
+                         d_conic, d_rgb):
+    """gs_render_backward_det: stores per instance, sums per splat in a fixed order, writes every gradient row."""
+    order, offsets, sorted_u, det_ws = det
+    _lib.call("gs_render_backward_det", B, P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(), ranges.data_ptr(),
+              ids_sorted.data_ptr(), _lib.ptr(sorted_u), order.data_ptr(), offsets.data_ptr(), final_T.data_ptr(),
+              n_contrib.data_ptr(), g_image.data_ptr(), _lib.ptr(seg), 0 if seg is None else seg.numel(),
+              _lib.ptr(det_ws), 0 if det_ws is None else det_ws.numel(), d_means2D.data_ptr(), d_conic.data_ptr(),
+              d_rgb.data_ptr(), _stream())
 
 
 def render_gaussians(means2D, conic_opacity, rgb, depths, radii, compute_locally, raster_settings, cuda_args=None,
-                     extended_compute_locally=None, *, tile_stats=False):
+                     extended_compute_locally=None, *, tile_stats=False, deterministic=None):
     """-> (image (3,H,W) with non-local tiles exactly 0, n_render, n_consider, n_contrib), and with tile_stats=True also
     (TILE_Y, TILE_X, 3) int64: per tile the list length, the entries walked and the entries blended summed over the tile's
     in-image pixels (gs_render_forward_ts; non-local tiles read 0).
+
+    deterministic: None follows torch.use_deterministic_algorithms.  When on and a gradient is needed, the backward
+    stores every (splat, tile) instance's gradient and sums them per splat in a fixed order (gs_render_backward_det):
+    two runs give the same bits.  The forward's outputs are bit-identical either way.
 
     cuda_args: the reference's dict.  On a logging iteration (statlog.request) zhx_time "True" appends stages 24-83 of
     this call and b10 of its backward to the gpu_time log, and zhx_debug "True" appends this call's per-tile lines and
@@ -474,7 +521,7 @@ def render_gaussians(means2D, conic_opacity, rgb, depths, radii, compute_locally
     if isinstance(cuda_args, dict):
         collector = cuda_args.setdefault("stats_collector", {})
     return _RenderGaussians.apply(means2D, conic_opacity, rgb, depths, radii, compute_locally, raster_settings, collector,
-                                  bool(tile_stats), statlog.request(cuda_args))
+                                  bool(tile_stats), statlog.request(cuda_args), deterministic_enabled(deterministic))
 
 
 MAX_VIEWS = 64   # GS_MAX_VIEWS
@@ -489,7 +536,7 @@ class _RenderGaussiansBatched(torch.autograd.Function):
     concatenated (camera k = rows [view_start[k], view_start[k+1])), masks (B,T), images (B,3,H,W)."""
 
     @staticmethod
-    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, view_start, rs, collector, want_ts):
+    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, view_start, rs, collector, want_ts, det):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         means2D, conic_opacity, rgb = _f32c(means2D, "means2D"), _f32c(conic_opacity, "conic_opacity"), _f32c(rgb, "rgb")
         depths = _f32c(depths, "depths")
@@ -531,28 +578,38 @@ class _RenderGaussiansBatched(torch.autograd.Function):
         stats = torch.empty((B, 3), dtype=torch.int64, device=dev)
         ts = torch.empty((B, ty, tx, 3), dtype=torch.int64, device=dev) if want_ts else None
         needs_grad = means2D.requires_grad or conic_opacity.requires_grad or rgb.requires_grad
+        det = det and needs_grad    # a forward-only render is the same bits either way
         R = C.c_int64(0)
         ticket = C.c_void_p()
         _lib.call("gs_render_count_launch", B, vs, P, H, W, means2D.data_ptr(), conic_opacity.data_ptr(), rgb.data_ptr(),
                   depths.data_ptr(), radii.data_ptr(), cl.data_ptr(), order.data_ptr(), offsets.data_ptr(),
                   rec.data_ptr(), temp.data_ptr(), tb, C.byref(ticket), s)
-        key = (B, H, W, needs_grad)
-        pre = _instance_buffers_before_sync(key, B * T, dev, needs_grad)   # host work while the count / sort / scan run
+        key = (B, H, W, needs_grad) if not det else (B, H, W, needs_grad, "det")
+        pre = _instance_buffers_before_sync(key, B * T, dev, needs_grad, det)   # host work while the count / sort / scan run
         _lib.call("gs_render_count_read", ticket, C.byref(R), s)    # the operator's one host sync
         R = int(R.value)
         global LAST_R_TOTAL
         LAST_R_TOTAL += R
-        ib = _instance_buffers_after_sync(key, pre, R, B * T, dev, needs_grad)
+        ib = _instance_buffers_after_sync(key, pre, R, B * T, dev, needs_grad, det)
         seg = ib.seg if R > 0 else None
-        _lib.call("gs_render_forward_batched_ts", B, vs, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
-                  order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
-                  ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(),
-                  image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts),
-                  _lib.ptr(seg), ib.segb if seg is not None else 0, s)
+        if det:
+            _lib.call("gs_render_forward_det", B, vs, P, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
+                      order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
+                      ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sorted_u.data_ptr(),
+                      ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(), image.data_ptr(), final_T.data_ptr(),
+                      n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts), _lib.ptr(seg),
+                      ib.segb if seg is not None else 0, s)
+        else:
+            _lib.call("gs_render_forward_batched_ts", B, vs, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
+                      order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
+                      ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(),
+                      image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts),
+                      _lib.ptr(seg), ib.segb if seg is not None else 0, s)
         ev1.record()
         _timed(collector, "forward_render_time", ev0, ev1)
         ids_sorted = ib.ids[1]    # a view: the (tile, id) scratch stays alive until the backward has run (16 B / instance)
         ctx.rs, ctx.R, ctx.P, ctx.B, ctx.collector, ctx.seg = rs, R, P, B, collector, seg
+        ctx.det = (order, offsets, ib.sorted_u, _det_workspace(ib, Pq, dev)) if det else None
         ctx.save_for_backward(rec, bg, cl, ranges, ids_sorted, final_T, n_contrib)
         if want_ts:
             ctx.mark_non_differentiable(stats, ts)
@@ -571,35 +628,40 @@ class _RenderGaussiansBatched(torch.autograd.Function):
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
         seg = ctx.seg
-        _lib.call("gs_render_backward_batched", B, P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(),
-                  ranges.data_ptr(), ids_sorted.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), g_image.data_ptr(),
-                  _lib.ptr(seg), 0 if seg is None else seg.numel(),
-                  d_means2D.data_ptr(), d_conic.data_ptr(), d_rgb.data_ptr(), _stream())
-        ctx.seg = None
+        if ctx.det is not None:
+            _render_backward_det(ctx.det, B, P, R, H, W, rec, bg, cl, ranges, ids_sorted, final_T, n_contrib, g_image, seg,
+                                 d_means2D, d_conic, d_rgb)
+        else:
+            _lib.call("gs_render_backward_batched", B, P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(),
+                      ranges.data_ptr(), ids_sorted.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), g_image.data_ptr(),
+                      _lib.ptr(seg), 0 if seg is None else seg.numel(),
+                      d_means2D.data_ptr(), d_conic.data_ptr(), d_rgb.data_ptr(), _stream())
+        ctx.seg = ctx.det = None
         ev1.record()
         _timed(ctx.collector, "backward_render_time", ev0, ev1)
-        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None, None
+        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None, None, None
 
 
 def render_gaussians_batched(means2D, conic_opacity, rgb, depths, radii, compute_locally, view_start, raster_settings,
-                             cuda_args=None, *, tile_stats=False):
+                             cuda_args=None, *, tile_stats=False, deterministic=None):
     """All B cameras of a batch in one pass.  means2D (N,2), conic_opacity (N,4), rgb (N,3), depths (N), radii (N):
     the splats of the B cameras concatenated, camera k = rows [view_start[k], view_start[k+1]) (len(view_start) = B+1);
     compute_locally (B, TILE_Y*TILE_X) (None = everything local); the cameras share the image size and background of
     `raster_settings` (their view / projection matrices were consumed by the preprocess).
     -> (images (B,3,H,W) with non-local tiles exactly 0, stats (B,3) int64 = n_render / n_consider / n_contrib), and
     with tile_stats=True also (B, TILE_Y, TILE_X, 3) int64: slice k is render_gaussians(..., tile_stats=True)'s for
-    camera k."""
+    camera k.  deterministic: as in render_gaussians."""
     collector = None
     if isinstance(cuda_args, dict):
         collector = cuda_args.setdefault("stats_collector", {})
     return _RenderGaussiansBatched.apply(means2D, conic_opacity, rgb, depths, radii, compute_locally,
-                                         [int(v) for v in view_start], raster_settings, collector, bool(tile_stats))
+                                         [int(v) for v in view_start], raster_settings, collector, bool(tile_stats),
+                                         deterministic_enabled(deterministic))
 
 
 class _FusedL1SSIMBatched(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, images, gts, rows4):
+    def forward(ctx, images, gts, rows4, det):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         images = _f32c(images, "images")
         B, _, H, W = images.shape
@@ -619,11 +681,12 @@ class _FusedL1SSIMBatched(torch.autograd.Function):
             keep.append(gt)
         flat = _i32_array([int(v) for r in rows4 for v in r])
         gptr = (C.c_void_p * B)(*[None if g is None else g.data_ptr() for g in keep])
-        tb = _lib.query("gs_loss_temp_bytes_batched", B, flat, W)
+        sfx = "_det" if det else ""
+        tb = _lib.query("gs_loss_temp_bytes_batched" + sfx, B, flat, W)
         temp = torch.empty((tb,), dtype=torch.uint8, device=images.device)
         out = torch.empty((B, 2), dtype=torch.float32, device=images.device)
-        _lib.call("gs_loss_forward_batched", B, H, W, flat, images.data_ptr(), gptr, out.data_ptr(), temp.data_ptr(), tb,
-                  _stream())
+        _lib.call("gs_loss_forward_batched" + sfx, B, H, W, flat, images.data_ptr(), gptr, out.data_ptr(), temp.data_ptr(),
+                  tb, _stream())
         ctx.rows4, ctx.gts = flat, keep
         ctx.save_for_backward(images, temp)
         return out
@@ -633,20 +696,23 @@ class _FusedL1SSIMBatched(torch.autograd.Function):
         images, temp = ctx.saved_tensors
         B, _, H, W = images.shape
         if g_out is None:
-            return None, None, None
+            return None, None, None, None
         g_l1, g_ssim = g_out[:, 0].to(torch.float32).contiguous(), g_out[:, 1].to(torch.float32).contiguous()
         d_images = torch.empty_like(images)
         gptr = (C.c_void_p * B)(*[None if g is None else g.data_ptr() for g in ctx.gts])
         _lib.call("gs_loss_backward_batched", B, H, W, ctx.rows4, images.data_ptr(), gptr, temp.data_ptr(),
                   g_l1.data_ptr(), g_ssim.data_ptr(), d_images.data_ptr(), _stream())
-        return d_images, None, None
+        return d_images, None, None, None
 
 
-def fused_l1_ssim_batched(images, gts_u8, rows4):
+def fused_l1_ssim_batched(images, gts_u8, rows4, *, deterministic=None):
     """The strip losses of the B cameras of a batch in one launch.  images (B,3,H,W); gts_u8: list of B CUDA uint8
     strips (3,rows,W) (None where rows == 0); rows4: B tuples (row0, row1, count_row0, count_row1).
-    -> (B,2) = (Ll1, ssim_loss) per camera, both normalised by 3*H*W; zeros for cameras without rows."""
-    return _FusedL1SSIMBatched.apply(images, list(gts_u8), [tuple(int(v) for v in r) for r in rows4])
+    -> (B,2) = (Ll1, ssim_loss) per camera, both normalised by 3*H*W; zeros for cameras without rows.
+    deterministic: None follows torch.use_deterministic_algorithms; when on, the per-CTA partial sums are added in a fixed
+    order (gs_loss_forward_batched_det), the same bits on every run."""
+    return _FusedL1SSIMBatched.apply(images, list(gts_u8), [tuple(int(v) for v in r) for r in rows4],
+                                     deterministic_enabled(deterministic))
 
 
 def get_local2j_ids_bool(image_height, image_width, rank, world_size, means2D, radii, dist_global_strategy,
@@ -689,7 +755,7 @@ class _FusedL1SSIM(torch.autograd.Function):
     """Per-strip (Ll1, ssim) of loss_distribution.py:2536-2585 in two kernels instead of ~20."""
 
     @staticmethod
-    def forward(ctx, image, gt_u8, row0, row1, crow0, crow1):
+    def forward(ctx, image, gt_u8, row0, row1, crow0, crow1, det):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         image = _f32c(image, "image")
         if gt_u8.dtype != torch.uint8 or not gt_u8.is_cuda:
@@ -699,11 +765,12 @@ class _FusedL1SSIM(torch.autograd.Function):
         rows = row1 - row0
         if tuple(gt_u8.shape) != (3, rows, W):
             raise ValueError(f"gt strip must be (3,{rows},{W}), got {tuple(gt_u8.shape)}")
-        tb = _lib.query("gs_loss_temp_bytes", rows, W)
+        sfx = "_det" if det else ""
+        tb = _lib.query("gs_loss_temp_bytes" + sfx, rows, W)
         temp = torch.empty((tb,), dtype=torch.uint8, device=image.device)
         out = torch.empty((2,), dtype=torch.float32, device=image.device)
-        _lib.call("gs_loss_forward", H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(), out.data_ptr(),
-                  temp.data_ptr(), tb, _stream())
+        _lib.call("gs_loss_forward" + sfx, H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
+                  out.data_ptr(), temp.data_ptr(), tb, _stream())
         ctx.rows = (row0, row1, crow0, crow1)
         ctx.save_for_backward(image, gt_u8, temp)
         return out[0], out[1]
@@ -720,17 +787,18 @@ class _FusedL1SSIM(torch.autograd.Function):
         d_image = torch.empty_like(image)
         _lib.call("gs_loss_backward", H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
                   temp.data_ptr(), g_l1.data_ptr(), g_ssim.data_ptr(), d_image.data_ptr(), _stream())
-        return d_image, None, None, None, None, None
+        return d_image, None, None, None, None, None, None
 
 
-def fused_l1_ssim(image, gt_u8, row0, row1, count_row0=None, count_row1=None):
+def fused_l1_ssim(image, gt_u8, row0, row1, count_row0=None, count_row1=None, *, deterministic=None):
     """-> (Ll1, ssim_loss) 0-dim tensors, both normalised by 3*H*W of the FULL image.
     Rows [row0,row1) of `image` (and the (3,row1-row0,W) uint8 `gt_u8`) form the window the 11x11 SSIM filter sees;
     only rows [count_row0,count_row1) (default: the whole window) are summed -- pass a window widened by exchanged halo
-    rows to make strip losses add up to the full-image loss (border-pixel exchange, loss_distribution.py:601-972)."""
+    rows to make strip losses add up to the full-image loss (border-pixel exchange, loss_distribution.py:601-972).
+    deterministic: as in fused_l1_ssim_batched."""
     c0 = int(row0) if count_row0 is None else int(count_row0)
     c1 = int(row1) if count_row1 is None else int(count_row1)
-    return _FusedL1SSIM.apply(image, gt_u8, int(row0), int(row1), c0, c1)
+    return _FusedL1SSIM.apply(image, gt_u8, int(row0), int(row1), c0, c1, deterministic_enabled(deterministic))
 
 
 _LOSS_W = {}
@@ -742,7 +810,7 @@ class _FusedLoss(torch.autograd.Function):
     product with a cached weight vector, and the backward hands (g (1 - lambda), -g lambda) to gs_loss_backward."""
 
     @staticmethod
-    def forward(ctx, image, gt_u8, row0, row1, crow0, crow1, lambda_dssim):
+    def forward(ctx, image, gt_u8, row0, row1, crow0, crow1, lambda_dssim, det):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         image = _f32c(image, "image")
         if gt_u8.dtype != torch.uint8 or not gt_u8.is_cuda:
@@ -756,11 +824,12 @@ class _FusedLoss(torch.autograd.Function):
         if key not in _LOSS_W:
             _LOSS_W[key] = torch.tensor([1.0 - lambda_dssim, -lambda_dssim], dtype=torch.float32, device=image.device)
         w = _LOSS_W[key]
-        tb = _lib.query("gs_loss_temp_bytes", rows, W)
+        sfx = "_det" if det else ""
+        tb = _lib.query("gs_loss_temp_bytes" + sfx, rows, W)
         temp = torch.empty((tb,), dtype=torch.uint8, device=image.device)
         out = torch.empty((2,), dtype=torch.float32, device=image.device)
-        _lib.call("gs_loss_forward", H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(), out.data_ptr(),
-                  temp.data_ptr(), tb, _stream())
+        _lib.call("gs_loss_forward" + sfx, H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
+                  out.data_ptr(), temp.data_ptr(), tb, _stream())
         ctx.rows, ctx.w = (row0, row1, crow0, crow1), w
         ctx.save_for_backward(image, gt_u8, temp)
         return torch.dot(out, w) + float(lambda_dssim)
@@ -771,20 +840,21 @@ class _FusedLoss(torch.autograd.Function):
         _, H, W = image.shape
         row0, row1, crow0, crow1 = ctx.rows
         if g is None:
-            return None, None, None, None, None, None, None
+            return None, None, None, None, None, None, None, None
         gw = (g.to(torch.float32) * ctx.w).contiguous()      # (g (1 - lambda), -g lambda)
         d_image = torch.empty_like(image)
         _lib.call("gs_loss_backward", H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
                   temp.data_ptr(), gw.data_ptr(), gw.data_ptr() + 4, d_image.data_ptr(), _stream())
-        return d_image, None, None, None, None, None, None
+        return d_image, None, None, None, None, None, None, None
 
 
-def fused_loss(image, gt_u8, row0, row1, lambda_dssim, count_row0=None, count_row1=None):
+def fused_loss(image, gt_u8, row0, row1, lambda_dssim, count_row0=None, count_row1=None, *, deterministic=None):
     """-> 0-dim loss (1 - lambda) Ll1 + lambda (1 - ssim) of the strip rows [row0, row1) (same window / count-row
-    semantics as fused_l1_ssim)."""
+    semantics as fused_l1_ssim; deterministic as in fused_l1_ssim_batched)."""
     c0 = int(row0) if count_row0 is None else int(count_row0)
     c1 = int(row1) if count_row1 is None else int(count_row1)
-    return _FusedLoss.apply(image, gt_u8, int(row0), int(row1), c0, c1, float(lambda_dssim))
+    return _FusedLoss.apply(image, gt_u8, int(row0), int(row1), c0, c1, float(lambda_dssim),
+                            deterministic_enabled(deterministic))
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -818,6 +888,14 @@ def get_pixels_compute_locally_and_in_rect(compute_locally, image_height, image_
     return out
 
 
+def _alert_scatter_add(caller):
+    """gs_image_tiles_scatter_add adds with float atomics where tile positions repeat: under
+    torch.use_deterministic_algorithms it raises (or warns, with warn_only=True) through torch's own alert, as index_add_
+    on CUDA does."""
+    from torch._prims_common import alert_not_deterministic
+    alert_not_deterministic(caller)
+
+
 class _LoadImageTilesByPos(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rect, pos, H, W, pixels_rect, tiles_rect):
@@ -840,6 +918,7 @@ class _LoadImageTilesByPos(torch.autograd.Function):
         if g is None:
             return None, None, None, None, None, None
         g = _f32c(g, "grad")
+        _alert_scatter_add("load_image_tiles_by_pos backward")
         out = torch.zeros((3, rh, rw), dtype=torch.float32, device=g.device)
         _lib.call("gs_image_tiles_scatter_add", pos.shape[0], pos.data_ptr(), g.data_ptr(), rh, rw, y0, x0, H, W,
                   out.data_ptr(), _stream())
@@ -850,6 +929,7 @@ class _MergeImageTilesByPos(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pos, tiles, H, W, pixels_rect, tiles_rect):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
+        _alert_scatter_add("merge_image_tiles_by_pos")
         tiles = _f32c(tiles, "tiles")
         pos = pos.to(device=tiles.device, dtype=torch.int64).contiguous().reshape(-1, 2)
         rh, rw = int(pixels_rect[1]) - int(pixels_rect[0]), int(pixels_rect[3]) - int(pixels_rect[2])

@@ -126,7 +126,7 @@ class Trainer:
     def __init__(self, scene, cams, gts_pinned, device, rank=0, world=1, lambda_dssim=0.2, group=None,
                  fused_activations=True, border_exchange=False, batched_render=True, peer_exchange=None,
                  peer_cap_rows=None, shard=None, load_balance=True, heuristic_decay=0.0,
-                 distributed_dataset_storage=False, feedback_lag=None, max_sh_degree=3):
+                 distributed_dataset_storage=False, feedback_lag=None, max_sh_degree=3, deterministic=False):
         """scene: the WHOLE scene (sliced here into this rank's contiguous shard), or -- shard=(lo, hi, n_total) -- only
         this rank's Gaussians [lo, hi) of an n_total-Gaussian scene (synthetic.make_scene_shard).
         load_balance: feed the measured render times back into the strip division after every step
@@ -139,7 +139,19 @@ class Trainer:
         step and cannot enqueue ahead).  > 0 (default 2, GS_B200_FEEDBACK_LAG) = the times of the step `feedback_lag`
         steps back, whose events have long completed, ride on the NEXT exchange's size all-gather (exchange.PIGGYBACK_IN):
         no collective of their own, no host sync; the strips move the same way, `feedback_lag` steps later.
-        max_sh_degree: the SH degree the model stores (GaussianParams)."""
+        max_sh_degree: the SH degree the model stores (GaussianParams).
+        deterministic: every render and loss of the step runs its atomic-free form (ops.render_gaussians(...,
+        deterministic=True)), so two runs of the same steps on the same inputs give the same bits in every loss, gradient
+        and, through FusedAdam and densification, parameter.  False leaves the choice to
+        torch.use_deterministic_algorithms.  This holds for a FIXED strip division: with more than one rank and
+        load_balance=True the strips follow measured render times, which differ from run to run, so that combination is
+        refused.  (The exchange sums gradients in a fixed rank order already; the NCCL all-reduce of replicated-Gaussian
+        gradient sync is outside this guarantee.)"""
+        if deterministic and world > 1 and load_balance:
+            raise ValueError("deterministic=True needs a fixed strip division: pass load_balance=False when world > 1 "
+                             "(the load balancer moves the strips by measured times)")
+        # None: the operators follow torch.use_deterministic_algorithms
+        self.deterministic = True if deterministic else None
         from . import exchange as _ex
         self._ex = _ex
         # splats travel by direct NVLink stores from the pack kernel and their gradients are pulled back over NVLink
@@ -389,7 +401,8 @@ class Trainer:
             cl, rows4, coef, const = self._bmask_cache[mk]
             m2, rgb, co, radii, depths = cat
             images, _stats = ops_.render_gaussians_batched(m2, co, rgb, depths, radii, cl, view_start, settings[0],
-                                                           {"stats_collector": collectors[0]})
+                                                           {"stats_collector": collectors[0]},
+                                                           deterministic=self.deterministic)
             self._n_renders = 1
             gts = []
             for k, (y0, y1, _c0, _c1) in enumerate(rows4):
@@ -402,7 +415,7 @@ class Trainer:
                     torch.cuda.current_stream().wait_event(ev)
                     gt.record_stream(torch.cuda.current_stream())
                     gts.append(gt)
-            l1_ssim = ops_.fused_l1_ssim_batched(images, gts, rows4)
+            l1_ssim = ops_.fused_l1_ssim_batched(images, gts, rows4, deterministic=self.deterministic)
             # sum over the local strips of (1 - lambda) Ll1 + lambda (1 - ssim)
             loss_sum = torch.dot(l1_ssim.reshape(-1), coef) + const
             Vp = int(view_start[-1])
@@ -421,12 +434,13 @@ class Trainer:
                 self._mask_cache[ck] = st.get_compute_locally(self.tile_x, self.device)
             cl = self._mask_cache[ck]
             image, *_ = ops_.render_gaussians(m2, co, rgb, depths, radii, cl, settings[k],
-                                              {"stats_collector": collectors[k]})
+                                              {"stats_collector": collectors[k]}, deterministic=self.deterministic)
             y0, y1 = st.local_pixel_rows(self.H)
             if self.border_exchange and self.world > 1 and len(st.gpu_ids) > 1:
                 from . import border
                 image, (r0, r1), _ = border.add_remote_border_rows(image, st, self.H, self.group)
-                loss = ops_.fused_loss(image, self.gts_dev[k][:, r0:r1, :].contiguous(), r0, r1, self.lambda_dssim, y0, y1)
+                loss = ops_.fused_loss(image, self.gts_dev[k][:, r0:r1, :].contiguous(), r0, r1, self.lambda_dssim, y0, y1,
+                                       deterministic=self.deterministic)
             else:
                 if resident:
                     gt = self._gt_strip(k, y0, y1, True)
@@ -434,7 +448,7 @@ class Trainer:
                     gt, ev = gt_ready[k]
                     torch.cuda.current_stream().wait_event(ev)
                     gt.record_stream(torch.cuda.current_stream())
-                loss = ops_.fused_loss(image, gt, y0, y1, self.lambda_dssim)
+                loss = ops_.fused_loss(image, gt, y0, y1, self.lambda_dssim, deterministic=self.deterministic)
             loss_sum = loss if loss_sum is None else loss_sum + loss
             Vp += m2.shape[0]
             Pl += (y1 - y0) * self.W

@@ -311,6 +311,39 @@ GS_API int gs_render_backward_batched(int num_views, int P, int64_t R, int image
                                       size_t seg_ws_bytes, float *dL_dmeans2D, float *dL_dconic_opacity, float *dL_drgb,
                                       void *stream);
 
+/* ---- deterministic render (torch.use_deterministic_algorithms) -- no reference counterpart -------------------------
+ * gs_render_backward adds each (splat, tile) instance's 9 gradient values into the splat's rows with float atomics, so
+ * their order -- and the last bits of every gradient -- depends on warp scheduling.  These calls replace
+ * gs_render_forward_batched_ts / gs_render_backward_batched when two runs must give the same bits:
+ *  - gs_render_forward_det: the same arguments as gs_render_forward_batched_ts (view_start_host may be NULL for one view
+ *    of P splats, as in gs_render_count_launch; P is ignored otherwise) plus sorted_u (R) uint32, which receives the
+ *    unsorted instance slot of every sorted entry.  ids_unsorted is written with the splat ids in unsorted order and
+ *    ids_sorted[r] = ids_unsorted[sorted_u[r]].  Every output (image, final_T, n_contrib, ranges, ids_sorted, stats,
+ *    tile_stats) is bit-identical to gs_render_forward_batched_ts's.  seg_ws may be NULL (forward only).
+ *  - gs_render_backward_det: stores each instance's 9 values at its slot of det_ws (gs_render_det_bytes(R, P) bytes,
+ *    256-byte aligned: 36 bytes per instance, 8 per splat), then sums every splat's slots [offsets[d-1], offsets[d])
+ *    (d = its depth position in order) in a fixed order -- one thread per splat, one CTA per splat with more than 16
+ *    instances -- and WRITES all three gradient outputs in full: no pre-initialisation.  order,
+ *    offsets: those of gs_render_count; seg_ws, sorted_u, ids_sorted: those the deterministic forward filled.  Needs the
+ *    segment workspace: without it, or with GS_DEBUG_BWD_TILE set, the call is refused (the tile-parallel kernel has no
+ *    deterministic form).  Results agree with gs_render_backward's up to summation order. */
+GS_API size_t gs_render_det_bytes(int64_t R, int P);
+GS_API int gs_render_forward_det(int num_views, const int32_t *view_start_host, int P, int64_t R, int image_height,
+                                 int image_width, const float *means2D, const int32_t *radii,
+                                 const uint8_t *compute_locally, const uint32_t *order, const uint32_t *offsets,
+                                 const float *rec, const float *bg, uint32_t *tiles_unsorted, uint32_t *ids_unsorted,
+                                 uint32_t *tiles_sorted, uint32_t *ids_sorted, uint32_t *sorted_u, void *sort_temp,
+                                 size_t sort_temp_bytes, uint32_t *ranges, float *image, float *final_T,
+                                 uint32_t *n_contrib, int64_t *stats, int64_t *tile_stats, void *seg_ws,
+                                 size_t seg_ws_bytes, void *stream);
+GS_API int gs_render_backward_det(int num_views, int P, int64_t R, int image_height, int image_width, const float *rec,
+                                  const float *bg, const uint8_t *compute_locally, const uint32_t *ranges,
+                                  const uint32_t *ids_sorted, const uint32_t *sorted_u, const uint32_t *order,
+                                  const uint32_t *offsets, const float *final_T, const uint32_t *n_contrib,
+                                  const float *dL_dimage, const void *seg_ws, size_t seg_ws_bytes, void *det_ws,
+                                  size_t det_ws_bytes, float *dL_dmeans2D, float *dL_dconic_opacity, float *dL_drgb,
+                                  void *stream);
+
 /* ---- per-kernel device timing ------------------------------------------------------------------
  * The reference's fork logs per-stage GPU times under --zhx_time ("10 preprocess time: 0.29 ms", ...;
  * /root/reference/analyze_statistic.py:1972-1991).  When enabled, every launch site brackets its
@@ -385,6 +418,20 @@ GS_API int gs_loss_forward_batched(int num_views, int image_height, int image_wi
 GS_API int gs_loss_backward_batched(int num_views, int image_height, int image_width, const int32_t *rows4_host,
                                     const float *image, const void *const *gt_u8_ptrs_host, const void *temp,
                                     const float *grad_l1, const float *grad_ssim, float *dL_dimage, void *stream);
+
+/* Deterministic forms of gs_loss_forward / gs_loss_forward_batched (no reference counterpart): those add one fp64 partial
+ * per CTA into the two sums with atomics, whose order varies from run to run; these write the partials to per-CTA slots
+ * and sum them in a fixed order, so the result is the same bits on every run (and within 1 ulp of fp32 of the atomic
+ * form).  Same arguments; temp is sized by the _det queries (8-byte aligned) and is read by the unchanged
+ * gs_loss_backward / gs_loss_backward_batched. */
+GS_API size_t gs_loss_temp_bytes_det(int rows, int image_width);
+GS_API int gs_loss_forward_det(int image_height, int image_width, int row0, int row1, int count_row0, int count_row1,
+                               const float *image, const uint8_t *gt_u8, float *out_l1_ssim, void *temp,
+                               size_t temp_bytes, void *stream);
+GS_API size_t gs_loss_temp_bytes_batched_det(int num_views, const int32_t *rows4_host, int image_width);
+GS_API int gs_loss_forward_batched_det(int num_views, int image_height, int image_width, const int32_t *rows4_host,
+                                       const float *image, const void *const *gt_u8_ptrs_host, float *out_l1_ssim,
+                                       void *temp, size_t temp_bytes, void *stream);
 
 /* ---- all-to-all staging -- gaussian_renderer/__init__.py:590-607,651-658 --------------------------
  * Replaces the per-(destination, camera) nonzero() + index_select + torch.cat glue around the sparse
