@@ -215,3 +215,66 @@ extern "C" int gs_densify_gather(int P, int S, int new_P, int num_tensors, const
     GS_LAUNCH_CHECK();
     return GS_OK;
 }
+
+// ---- densification statistics: the reference's densification.py:15-24 + scene/gaussian_model.py:1046-1052 ----------
+// Per camera k of the batch, in batch order, over the Gaussians with radii_k > 0:
+//     max_radii2D = torch.max(max_radii2D, radii_k);  xyz_gradient_accum += ||means2D_k.grad[:, :2]||;  denom += 1
+// Every masked read / write there is a nonzero (a host sync).  Here one thread per Gaussian walks the views in the same
+// order, so the fp32 sum is the reference's sequence; rows visible in no view are neither loaded nor stored.
+struct DsViews {
+    const float2 *grad[GS_MAX_VIEWS];
+    const int32_t *radii[GS_MAX_VIEWS];
+};
+
+// torch.norm(g, dim=-1) of a 2-vector on the device: the two squares are rounded, then summed (tests/
+// test_densify_stats_gpu.py, test_norm_form, checks this against torch on inputs where the FMA forms differ)
+GS_D float ds_norm(float2 g) { return __fsqrt_rn(__fadd_rn(__fmul_rn(g.x, g.x), __fmul_rn(g.y, g.y))); }
+
+__global__ void __launch_bounds__(DN_THREADS)
+k_densify_stats(int B, int P, const DsViews v, float *__restrict__ accum, float *__restrict__ denom,
+                float *__restrict__ max_radii) {
+    const int i = blockIdx.x * DN_THREADS + threadIdx.x;
+    if (i >= P) return;
+    float a = 0.f, d = 0.f, m = 0.f;
+    bool seen = false;
+    for (int k = 0; k < B; k++) {
+        const int r = v.radii[k][i];
+        if (r <= 0) continue;                              // visibility_filter = radii > 0
+        const float2 g = v.grad[k][i];
+        if (!seen) {
+            a = accum[i]; d = denom[i]; m = max_radii[i];
+            seen = true;
+        }
+        const float f = __int2float_rn(r);                 // torch's int32 -> float32 promotion rounds to nearest
+        m = (isnan(m) || m > f) ? m : f;                   // torch.max: a NaN operand is returned as is
+        a = __fadd_rn(a, ds_norm(g));
+        d = __fadd_rn(d, 1.f);
+    }
+    if (seen) {
+        accum[i] = a; denom[i] = d; max_radii[i] = m;
+    }
+}
+
+extern "C" int gs_densify_stats(int num_views, int P, const void *const *grad_host, const void *const *radii_host,
+                                float *xyz_gradient_accum, float *denom, float *max_radii2D, void *stream) {
+    GS_REQUIRE(num_views >= 1 && num_views <= GS_MAX_VIEWS, "num_views");
+    GS_REQUIRE(P >= 0, "P");
+    GS_REQUIRE(grad_host && radii_host && xyz_gradient_accum && denom && max_radii2D, "null pointer");
+    DsViews v;
+    for (int k = 0; k < GS_MAX_VIEWS; k++) {
+        const bool in = k < num_views;
+        v.grad[k] = in ? (const float2 *)grad_host[k] : nullptr;
+        v.radii[k] = in ? (const int32_t *)radii_host[k] : nullptr;
+        if (!in) continue;
+        GS_REQUIRE(v.grad[k] && v.radii[k], "null pointer");
+        GS_REQUIRE(((uintptr_t)v.grad[k] & 7) == 0, "means2D gradients must be 8-byte aligned (float2 loads)");
+        GS_REQUIRE(((uintptr_t)v.radii[k] & 3) == 0, "radii must be 4-byte aligned");
+    }
+    GS_REQUIRE((((uintptr_t)xyz_gradient_accum | (uintptr_t)denom | (uintptr_t)max_radii2D) & 3) == 0,
+               "statistics must be 4-byte aligned");
+    if (P == 0) return GS_OK;
+    k_densify_stats<<<(P + DN_THREADS - 1) / DN_THREADS, DN_THREADS, 0, (cudaStream_t)stream>>>(
+        num_views, P, v, xyz_gradient_accum, denom, max_radii2D);
+    GS_LAUNCH_CHECK();
+    return GS_OK;
+}

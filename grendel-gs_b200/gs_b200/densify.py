@@ -16,6 +16,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from .ops import MAX_VIEWS
 
 NAMES = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation")
 KIND = {"xyz": 1, "scaling": 2}   # 0 copy, 1 position, 2 log-scale, 3 Adam moment (include/grendel_gs_b200.h)
@@ -107,6 +108,59 @@ def densify_and_prune(optimizer, xyz_gradient_accum, denom, max_grad, min_opacit
         result["send_to_gpui_cnt"] = outs["send_to_gpui_cnt"]
     result["counts"] = (kept, clones, child1, S, new_P)
     return result
+
+
+def _check(t, name, dtype, shape):
+    """Refuse anything but a contiguous tensor of `dtype` and `shape` (None in `shape`: any size)."""
+    if t is None:
+        raise TypeError(f"{name} is None (no gradient was retained for this camera?)")
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name} must be a tensor, got {type(t).__name__}")
+    if t.dtype != dtype:
+        raise TypeError(f"{name} must be {dtype}, got {t.dtype}")
+    if t.dim() != len(shape) or any(want is not None and got != want for got, want in zip(t.shape, shape)):
+        raise ValueError(f"{name} must be {tuple('P' if d is None else d for d in shape)}, got {tuple(t.shape)}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+
+
+def add_densification_stats(xyz_gradient_accum, denom, max_radii2D, means2D_grads, radii):
+    """The densification statistics of one step, updated in place on the current stream by one launch with no host
+    synchronisation (gs_densify_stats).  The reference's loop (densification.py:15-24 with
+    GaussianModel.add_densification_stats, scene/gaussian_model.py:1046-1052), bit for bit: for each camera k in batch
+    order, where radii[k] > 0,
+        max_radii2D = torch.max(max_radii2D, radii[k]);  xyz_gradient_accum += norm(means2D_grads[k]);  denom += 1.
+    xyz_gradient_accum, denom: (P, 1) float32; max_radii2D: (P,) float32 (the reference's layout, which
+    densify_and_prune's reset statistics have).  means2D_grads: (B, P, 2) float32 or a list of B (P, 2) (each camera's
+    means2D.grad); radii: (B, P) int32 or a list of B (P,).  1 <= B <= 64.  Nothing is made contiguous or converted here:
+    other inputs are refused (ValueError / TypeError)."""
+    if means2D_grads is None or radii is None:
+        raise TypeError("means2D_grads and radii are required (no gradient was retained?)")
+    grads =list(means2D_grads.unbind(0)) if isinstance(means2D_grads, torch.Tensor) else list(means2D_grads)
+    rads = list(radii.unbind(0)) if isinstance(radii, torch.Tensor) else list(radii)
+    B = len(grads)
+    if not 1 <= B <= MAX_VIEWS:
+        raise ValueError(f"between 1 and {MAX_VIEWS} views, got {B}")
+    if len(rads) != B:
+        raise ValueError(f"{B} gradient views but {len(rads)} radii views")
+    P = xyz_gradient_accum.shape[0] if isinstance(xyz_gradient_accum, torch.Tensor) else None
+    for name, t, shape in (("xyz_gradient_accum", xyz_gradient_accum, (P, 1)), ("denom", denom, (P, 1)),
+                           ("max_radii2D", max_radii2D, (P,))):
+        _check(t, name, torch.float32, shape)
+    for k in range(B):
+        _check(grads[k], f"means2D_grads[{k}]", torch.float32, (P, 2))
+        _check(rads[k], f"radii[{k}]", torch.int32, (P,))
+    dev = xyz_gradient_accum.device
+    for t in [xyz_gradient_accum, denom, max_radii2D] + grads + rads:
+        if not t.is_cuda:
+            raise TypeError("add_densification_stats needs CUDA tensors (no CPU path)")
+        if t.device != dev:
+            raise ValueError("all tensors must be on one device")
+    vp = C.c_void_p * B
+    with torch.cuda.device(dev):
+        _lib.call("gs_densify_stats", B, P, vp(*[t.data_ptr() for t in grads]), vp(*[t.data_ptr() for t in rads]),
+                  xyz_gradient_accum.data_ptr(), denom.data_ptr(), max_radii2D.data_ptr(),
+                  torch.cuda.current_stream(dev).cuda_stream)
 
 
 def append_gaussians(optimizer, new_tensors):

@@ -526,6 +526,15 @@ class Trainer:
         times = allt.reshape(self.world, B).cpu().tolist()       # gpu_camera_running_time[gpu][camera]
         finish_strategy(self.history, strategies, times, self.iteration, self.world, self.H, self.W, self.heuristic_decay)
 
+    def add_densification_stats(self, xyz_gradient_accum, denom, max_radii2D):
+        """The densification statistics of the last step (densification.py:15-24), in place, one launch, no host sync:
+        densify.add_densification_stats over this rank's screen-space gradients and pre-exchange radii of every camera of
+        the step (the reference's batched_locally_preprocessed_mean2D / _radii), whichever of the batched or per-camera
+        preprocess the step ran.  xyz_gradient_accum, denom: (P, 1), max_radii2D: (P,), float32, P = n_local."""
+        from . import densify
+        grads = self.means2D.grad if isinstance(self.means2D, torch.Tensor) else [m.grad for m in self.means2D]
+        densify.add_densification_stats(xyz_gradient_accum, denom, max_radii2D, grads, self._radii_local)
+
     GROUP_OF = {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity",
                 "scaling": "_scaling", "rotation": "_rotation"}
 

@@ -568,6 +568,17 @@ GS_API int gs_densify_select(int P, const float *xyz_gradient_accum, const float
 GS_API int gs_densify_gather(int P, int S, int new_P, int num_tensors, const void *const *src_host, void *const *dst_host,
                              const int32_t *width_host, const int32_t *kind_host, const float *scaling_raw,
                              const float *rotation_raw, const float *noise, const void *temp, void *stream);
+/* Densification statistics of one step (densification.py:15-24, scene/gaussian_model.py:1046-1052): for each view k =
+ * 0 .. num_views-1 IN BATCH ORDER and each Gaussian i with radii_k[i] > 0,
+ *     max_radii2D[i]        = max(max_radii2D[i], float(radii_k[i]))      (int32 -> fp32 rounded to nearest; NaN kept)
+ *     xyz_gradient_accum[i] = xyz_gradient_accum[i] + sqrt(rn(gx^2) + rn(gy^2))     (gx, gy = grad_k[i], torch.norm)
+ *     denom[i]              = denom[i] + 1
+ * in fp32, one rounding per operation: the reference's per-camera masked updates, bit for bit.  Rows visible in no view
+ * are not written.  grad_host / radii_host: HOST arrays of num_views (1..GS_MAX_VIEWS) device pointers to (P,2) fp32
+ * screen-space gradients (8-byte aligned) and (P) int32 radii; the three statistics are (P) fp32 (4-byte aligned),
+ * updated in place.  One launch, no atomics, no host synchronisation; P == 0 launches nothing. */
+GS_API int gs_densify_stats(int num_views, int P, const void *const *grad_host, const void *const *radii_host,
+                            float *xyz_gradient_accum, float *denom, float *max_radii2D, void *stream);
 
 /* ---- simple_knn._C.distCUDA2 -- /root/reference/scene/gaussian_model.py:20,163-166 ------------------------------------
  * Mean squared distance of every point to its 3 nearest OTHER points (self excluded by index, duplicates count at
