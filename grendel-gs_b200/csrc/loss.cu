@@ -41,7 +41,7 @@ extern "C" size_t gs_loss_temp_bytes(int rows, int image_width) {
 struct LossViews {
     int row0[GS_MAX_VIEWS], rows[GS_MAX_VIEWS];       // window rows [row0, row0+rows) of the view's image
     int crow0[GS_MAX_VIEWS], crow1[GS_MAX_VIEWS];     // counted rows, relative to row0
-    const uint8_t *gt[GS_MAX_VIEWS];                  // (3, rows, W) uint8 ground truth of the window
+    const uint8_t *gt[GS_MAX_VIEWS];                  // (3, rows, W) uint8 ground truth of the window (GT_FULL: (3, H, W))
     unsigned long long map_off[GS_MAX_VIEWS];         // float offset of the view's 9 derivative planes in `maps`
 };
 
@@ -49,7 +49,9 @@ struct LossViews {
 // DET (deterministic loss): each CTA writes its two fp64 partials to its own slot of `partials` (CTA (x, y) of view v:
 // slot (v gridDim.y + y) gridDim.x + x; CTAs below the view's strip write zeros) instead of adding them atomically into
 // `sums`; k_loss_finalize_det sums the slots in a fixed order.
-template <bool DET>
+// GT_FULL: lv.gt[v] is the view's whole (3, H, W) ground-truth image, read in place at rows [row0, row0+rows) with channel
+// pitch H W; otherwise it is the (3, rows, W) strip of those rows (channel pitch rows W).
+template <bool DET, bool GT_FULL>
 __global__ void __launch_bounds__(LS_THREADS)
 k_loss_fwd(int W, int H, const LossViews lv, const float *__restrict__ image, float *__restrict__ maps,
            double *__restrict__ sums, double *__restrict__ partials) {
@@ -65,8 +67,8 @@ k_loss_fwd(int W, int H, const LossViews lv, const float *__restrict__ image, fl
             if (threadIdx.x == 0) { partials[0] = 0.0; partials[1] = 0.0; }
         return;
     }
-    const size_t HW = (size_t)H * W, SW = (size_t)rows * W;
-    const uint8_t *__restrict__ gt = lv.gt[view];
+    const size_t HW = (size_t)H * W, SW = (size_t)rows * W, GS = GT_FULL ? HW : SW;
+    const uint8_t *__restrict__ gt = lv.gt[view] + (GT_FULL ? (size_t)row0 * W : 0);
     image += (size_t)view * 3 * HW;
     maps += lv.map_off[view];
     sums += 2 * view;
@@ -79,7 +81,7 @@ k_loss_fwd(int W, int H, const LossViews lv, const float *__restrict__ image, fl
             float vx = 0.f, vy = 0.f;
             if (y >= 0 && y < rows && x >= 0 && x < W) {
                 vx = image[ch * HW + (size_t)(row0 + y) * W + x];
-                vy = fminf(1.f, fmaxf(0.f, (float)gt[ch * SW + (size_t)y * W + x] / 255.0f));
+                vy = fminf(1.f, fmaxf(0.f, (float)gt[ch * GS + (size_t)y * W + x] / 255.0f));
             }
             s_x[r][c] = vx; s_y[r][c] = vy;
         }
@@ -176,6 +178,7 @@ k_loss_finalize_det(int slots, const double *__restrict__ partials, double inv_n
     if (lane == 0) out[2 * view + w] = (float)(s * inv_norm);
 }
 
+template <bool GT_FULL>
 __global__ void __launch_bounds__(LS_THREADS)
 k_loss_bwd(int W, int H, const LossViews lv, const float *__restrict__ image, const float *__restrict__ maps,
            const float *__restrict__ grad_l1, const float *__restrict__ grad_ssim, float inv_norm,
@@ -186,8 +189,8 @@ k_loss_bwd(int W, int H, const LossViews lv, const float *__restrict__ image, co
     const int row0 = lv.row0[view], rows = lv.rows[view], crow0 = lv.crow0[view], crow1 = lv.crow1[view];
     const int tx0 = blockIdx.x * LS_TILE, ty0 = blockIdx.y * LS_TILE;
     if (ty0 >= rows) return;
-    const size_t HW = (size_t)H * W, SW = (size_t)rows * W;
-    const uint8_t *__restrict__ gt = lv.gt[view];
+    const size_t HW = (size_t)H * W, SW = (size_t)rows * W, GS = GT_FULL ? HW : SW;
+    const uint8_t *__restrict__ gt = lv.gt[view] + (GT_FULL ? (size_t)row0 * W : 0);
     image += (size_t)view * 3 * HW;
     dimg += (size_t)view * 3 * HW;
     maps += lv.map_off[view];
@@ -241,7 +244,7 @@ k_loss_bwd(int W, int H, const LossViews lv, const float *__restrict__ image, co
                 if (y < rows && x < W) {
                     const size_t oi = ch * HW + (size_t)(row0 + y) * W + x;
                     const float vx = image[oi];
-                    const float vy = fminf(1.f, fmaxf(0.f, (float)gt[ch * SW + (size_t)y * W + x] / 255.0f));
+                    const float vy = fminf(1.f, fmaxf(0.f, (float)gt[ch * GS + (size_t)y * W + x] / 255.0f));
                     const float d = vx - vy;
                     const float sgn = (y < crow0 || y >= crow1) ? 0.f : (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f));
                     dimg[oi] = gl1 * sgn + gss * (b0[q] + 2.f * vx * b1[q] + vy * b2[q]);
@@ -258,8 +261,9 @@ k_loss_bwd(int W, int H, const LossViews lv, const float *__restrict__ image, co
 
 // rows4: (num_views, 4) HOST ints = row0, row1, count_row0, count_row1 per view; row1 == row0 skips the view.
 // Fills the kernel-side table; returns the tallest window in *max_rows and the total window rows in *sum_rows.
-static int make_loss_views(int num_views, int H, int W, const int32_t *rows4, const void *const *gts, LossViews &lv,
-                           int *max_rows, size_t *sum_rows) {
+// gt_full: gts[v] are whole (3, H, W) images, which start an allocation: a pointer off a 16-byte boundary is refused.
+static int make_loss_views(int num_views, int H, int W, const int32_t *rows4, const void *const *gts, bool gt_full,
+                           LossViews &lv, int *max_rows, size_t *sum_rows) {
     GS_REQUIRE(num_views >= 1 && num_views <= GS_MAX_VIEWS, "num_views must be in [1, GS_MAX_VIEWS]");
     GS_REQUIRE(H > 0 && W > 0 && rows4 && gts, "sizes");
     size_t off = 0;
@@ -275,6 +279,7 @@ static int make_loss_views(int num_views, int H, int W, const int32_t *rows4, co
         if (rows == 0) continue;
         GS_REQUIRE(c0 >= row0 && c1 <= row1 && c1 >= c0, "count rows must lie inside [row0,row1)");
         GS_REQUIRE(gts[v] != nullptr, "null ground-truth pointer");
+        GS_REQUIRE(!gt_full || ((uintptr_t)gts[v] & 15) == 0, "full ground-truth image must be 16-byte aligned");
         lv.row0[v] = row0; lv.rows[v] = rows; lv.crow0[v] = c0 - row0; lv.crow1[v] = c1 - row0;
         lv.gt[v] = (const uint8_t *)gts[v];
         lv.map_off[v] = (unsigned long long)off;
@@ -294,12 +299,13 @@ static size_t det_slot_bytes(int num_views, int max_rows, int W) {
 }
 
 static int loss_forward_impl(int num_views, int H, int W, const int32_t *rows4, const float *image, const void *const *gts,
-                             float *out, void *temp, size_t temp_bytes, size_t header, bool det, cudaStream_t stream) {
+                             float *out, void *temp, size_t temp_bytes, size_t header, bool det, bool gt_full,
+                             cudaStream_t stream) {
     GS_REQUIRE(image && out && temp, "null pointer");
     LossViews lv;
     int max_rows = 0;
     size_t sum_rows = 0;
-    int rc = make_loss_views(num_views, H, W, rows4, gts, lv, &max_rows, &sum_rows);
+    int rc = make_loss_views(num_views, H, W, rows4, gts, gt_full, lv, &max_rows, &sum_rows);
     if (rc != GS_OK) return rc;
     const size_t need = det ? header + det_maps_bytes(sum_rows, W) + det_slot_bytes(num_views, max_rows, W)
                             : header + (size_t)9 * sum_rows * W * sizeof(float);
@@ -319,7 +325,8 @@ static int loss_forward_impl(int num_views, int H, int W, const int32_t *rows4, 
         const int gy = (max_rows + LS_TILE - 1) / LS_TILE, gxl = (W + LS_TILE - 1) / LS_TILE;
         if (max_rows > 0) {
             dim3 grid(gxl, gy, num_views);
-            k_loss_fwd<true><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, nullptr, partials);
+            if (gt_full) k_loss_fwd<true, true><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, nullptr, partials);
+            else k_loss_fwd<true, false><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, nullptr, partials);
             GS_LAUNCH_CHECK();
         }
         k_loss_finalize_det<<<num_views, 64, 0, stream>>>(gxl * gy, partials, inv_norm, out);
@@ -330,7 +337,8 @@ static int loss_forward_impl(int num_views, int H, int W, const int32_t *rows4, 
     GsStageTimer timer(GS_STAGE_LOSS_FWD, stream);
     if (max_rows > 0) {
         dim3 grid((W + LS_TILE - 1) / LS_TILE, (max_rows + LS_TILE - 1) / LS_TILE, num_views);
-        k_loss_fwd<false><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, sums, nullptr);
+        if (gt_full) k_loss_fwd<false, true><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, sums, nullptr);
+        else k_loss_fwd<false, false><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, sums, nullptr);
         GS_LAUNCH_CHECK();
     }
     k_loss_finalize<<<1, 2 * GS_MAX_VIEWS, 0, stream>>>(num_views, sums, inv_norm, out);
@@ -340,12 +348,12 @@ static int loss_forward_impl(int num_views, int H, int W, const int32_t *rows4, 
 
 static int loss_backward_impl(int num_views, int H, int W, const int32_t *rows4, const float *image,
                               const void *const *gts, const void *temp, const float *grad_l1, const float *grad_ssim,
-                              float *dimg, size_t header, cudaStream_t stream) {
+                              float *dimg, size_t header, bool gt_full, cudaStream_t stream) {
     GS_REQUIRE(image && temp && grad_l1 && grad_ssim && dimg, "null pointer");
     LossViews lv;
     int max_rows = 0;
     size_t sum_rows = 0;
-    int rc = make_loss_views(num_views, H, W, rows4, gts, lv, &max_rows, &sum_rows);
+    int rc = make_loss_views(num_views, H, W, rows4, gts, gt_full, lv, &max_rows, &sum_rows);
     if (rc != GS_OK) return rc;
     rc = ensure_gauss();
     if (rc != GS_OK) return rc;
@@ -365,8 +373,9 @@ static int loss_backward_impl(int num_views, int H, int W, const int32_t *rows4,
     if (max_rows == 0) return GS_OK;
     dim3 grid((W + LS_TILE - 1) / LS_TILE, (max_rows + LS_TILE - 1) / LS_TILE, num_views);
     GsStageTimer timer(GS_STAGE_LOSS_BWD, stream);
-    k_loss_bwd<<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, grad_l1, grad_ssim,
-                                                (float)(1.0 / (3.0 * (double)H * (double)W)), dimg);
+    const float inv_norm = (float)(1.0 / (3.0 * (double)H * (double)W));
+    if (gt_full) k_loss_bwd<true><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, grad_l1, grad_ssim, inv_norm, dimg);
+    else k_loss_bwd<false><<<grid, LS_THREADS, 0, stream>>>(W, H, lv, image, maps, grad_l1, grad_ssim, inv_norm, dimg);
     GS_LAUNCH_CHECK();
     return GS_OK;
 }
@@ -379,7 +388,7 @@ extern "C" int gs_loss_forward(int image_height, int image_width, int row0, int 
     const int32_t rows4[4] = {row0, row1, count_row0, count_row1};
     const void *gts[1] = {gt_u8};
     return loss_forward_impl(1, image_height, image_width, rows4, image, gts, out_l1_ssim, temp, temp_bytes, LS_HEADER_1,
-                             false, (cudaStream_t)stream_);
+                             false, false, (cudaStream_t)stream_);
 }
 
 extern "C" size_t gs_loss_temp_bytes_det(int rows, int image_width) {
@@ -395,7 +404,7 @@ extern "C" int gs_loss_forward_det(int image_height, int image_width, int row0, 
     const int32_t rows4[4] = {row0, row1, count_row0, count_row1};
     const void *gts[1] = {gt_u8};
     return loss_forward_impl(1, image_height, image_width, rows4, image, gts, out_l1_ssim, temp, temp_bytes, LS_HEADER_1,
-                             true, (cudaStream_t)stream_);
+                             true, false, (cudaStream_t)stream_);
 }
 
 extern "C" size_t gs_loss_temp_bytes_batched(int num_views, const int32_t *rows4_host, int image_width) {
@@ -411,7 +420,7 @@ extern "C" int gs_loss_forward_batched(int num_views, int image_height, int imag
                                        const float *image, const void *const *gt_u8_ptrs_host, float *out_l1_ssim,
                                        void *temp, size_t temp_bytes, void *stream_) {
     return loss_forward_impl(num_views, image_height, image_width, rows4_host, image, gt_u8_ptrs_host, out_l1_ssim, temp,
-                             temp_bytes, LS_HEADER_B, false, (cudaStream_t)stream_);
+                             temp_bytes, LS_HEADER_B, false, false, (cudaStream_t)stream_);
 }
 
 extern "C" size_t gs_loss_temp_bytes_batched_det(int num_views, const int32_t *rows4_host, int image_width) {
@@ -430,7 +439,7 @@ extern "C" int gs_loss_forward_batched_det(int num_views, int image_height, int 
                                            const float *image, const void *const *gt_u8_ptrs_host, float *out_l1_ssim,
                                            void *temp, size_t temp_bytes, void *stream_) {
     return loss_forward_impl(num_views, image_height, image_width, rows4_host, image, gt_u8_ptrs_host, out_l1_ssim, temp,
-                             temp_bytes, LS_HEADER_B, true, (cudaStream_t)stream_);
+                             temp_bytes, LS_HEADER_B, true, false, (cudaStream_t)stream_);
 }
 
 extern "C" int gs_loss_backward(int image_height, int image_width, int row0, int row1, int count_row0, int count_row1,
@@ -441,12 +450,37 @@ extern "C" int gs_loss_backward(int image_height, int image_width, int row0, int
     const int32_t rows4[4] = {row0, row1, count_row0, count_row1};
     const void *gts[1] = {gt_u8};
     return loss_backward_impl(1, image_height, image_width, rows4, image, gts, temp, grad_l1, grad_ssim, dL_dimage,
-                              LS_HEADER_1, (cudaStream_t)stream_);
+                              LS_HEADER_1, false, (cudaStream_t)stream_);
 }
 
 extern "C" int gs_loss_backward_batched(int num_views, int image_height, int image_width, const int32_t *rows4_host,
                                         const float *image, const void *const *gt_u8_ptrs_host, const void *temp,
                                         const float *grad_l1, const float *grad_ssim, float *dL_dimage, void *stream_) {
     return loss_backward_impl(num_views, image_height, image_width, rows4_host, image, gt_u8_ptrs_host, temp, grad_l1,
-                              grad_ssim, dL_dimage, LS_HEADER_B, (cudaStream_t)stream_);
+                              grad_ssim, dL_dimage, LS_HEADER_B, false, (cudaStream_t)stream_);
+}
+
+// The batched entry points with each view's ground truth as its whole (3, H, W) image, read in place: temp is sized by
+// gs_loss_temp_bytes_batched / _det as for the strip forms.
+extern "C" int gs_loss_forward_batched_gt_full(int num_views, int image_height, int image_width, const int32_t *rows4_host,
+                                               const float *image, const void *const *gt_u8_ptrs_host, float *out_l1_ssim,
+                                               void *temp, size_t temp_bytes, void *stream_) {
+    return loss_forward_impl(num_views, image_height, image_width, rows4_host, image, gt_u8_ptrs_host, out_l1_ssim, temp,
+                             temp_bytes, LS_HEADER_B, false, true, (cudaStream_t)stream_);
+}
+
+extern "C" int gs_loss_forward_batched_gt_full_det(int num_views, int image_height, int image_width,
+                                                   const int32_t *rows4_host, const float *image,
+                                                   const void *const *gt_u8_ptrs_host, float *out_l1_ssim, void *temp,
+                                                   size_t temp_bytes, void *stream_) {
+    return loss_forward_impl(num_views, image_height, image_width, rows4_host, image, gt_u8_ptrs_host, out_l1_ssim, temp,
+                             temp_bytes, LS_HEADER_B, true, true, (cudaStream_t)stream_);
+}
+
+extern "C" int gs_loss_backward_batched_gt_full(int num_views, int image_height, int image_width, const int32_t *rows4_host,
+                                                const float *image, const void *const *gt_u8_ptrs_host, const void *temp,
+                                                const float *grad_l1, const float *grad_ssim, float *dL_dimage,
+                                                void *stream_) {
+    return loss_backward_impl(num_views, image_height, image_width, rows4_host, image, gt_u8_ptrs_host, temp, grad_l1,
+                              grad_ssim, dL_dimage, LS_HEADER_B, true, (cudaStream_t)stream_);
 }

@@ -661,12 +661,13 @@ def render_gaussians_batched(means2D, conic_opacity, rgb, depths, radii, compute
 
 class _FusedL1SSIMBatched(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, images, gts, rows4, det):
+    def forward(ctx, images, gts, rows4, det, gt_full):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         images = _f32c(images, "images")
         B, _, H, W = images.shape
         if len(gts) != B or len(rows4) != B:
             raise ValueError("one ground-truth strip and one (row0,row1,count_row0,count_row1) per view")
+        what = "images (3, H, W)" if gt_full else "strips (3, rows, W)"
         keep = []
         for k, (gt, r) in enumerate(zip(gts, rows4)):
             rows = int(r[1]) - int(r[0])
@@ -674,10 +675,11 @@ class _FusedL1SSIMBatched(torch.autograd.Function):
                 keep.append(None)
                 continue
             if gt is None or gt.dtype != torch.uint8 or not gt.is_cuda:
-                raise TypeError("gt strips must be CUDA uint8 tensors (3, rows, W)")
+                raise TypeError(f"gt {what} must be CUDA uint8 tensors")
             gt = gt.contiguous()
-            if tuple(gt.shape) != (3, rows, W):
-                raise ValueError(f"gt strip {k} must be (3,{rows},{W}), got {tuple(gt.shape)}")
+            want = (3, H, W) if gt_full else (3, rows, W)
+            if tuple(gt.shape) != want:
+                raise ValueError(f"gt {k} must be {want}, got {tuple(gt.shape)}")
             keep.append(gt)
         flat = _i32_array([int(v) for r in rows4 for v in r])
         gptr = (C.c_void_p * B)(*[None if g is None else g.data_ptr() for g in keep])
@@ -685,9 +687,10 @@ class _FusedL1SSIMBatched(torch.autograd.Function):
         tb = _lib.query("gs_loss_temp_bytes_batched" + sfx, B, flat, W)
         temp = torch.empty((tb,), dtype=torch.uint8, device=images.device)
         out = torch.empty((B, 2), dtype=torch.float32, device=images.device)
-        _lib.call("gs_loss_forward_batched" + sfx, B, H, W, flat, images.data_ptr(), gptr, out.data_ptr(), temp.data_ptr(),
-                  tb, _stream())
-        ctx.rows4, ctx.gts = flat, keep
+        full = "_gt_full" if gt_full else ""
+        _lib.call("gs_loss_forward_batched" + full + sfx, B, H, W, flat, images.data_ptr(), gptr, out.data_ptr(),
+                  temp.data_ptr(), tb, _stream())
+        ctx.rows4, ctx.gts, ctx.full = flat, keep, full
         ctx.save_for_backward(images, temp)
         return out
 
@@ -696,23 +699,25 @@ class _FusedL1SSIMBatched(torch.autograd.Function):
         images, temp = ctx.saved_tensors
         B, _, H, W = images.shape
         if g_out is None:
-            return None, None, None, None
+            return None, None, None, None, None
         g_l1, g_ssim = g_out[:, 0].to(torch.float32).contiguous(), g_out[:, 1].to(torch.float32).contiguous()
         d_images = torch.empty_like(images)
         gptr = (C.c_void_p * B)(*[None if g is None else g.data_ptr() for g in ctx.gts])
-        _lib.call("gs_loss_backward_batched", B, H, W, ctx.rows4, images.data_ptr(), gptr, temp.data_ptr(),
+        _lib.call("gs_loss_backward_batched" + ctx.full, B, H, W, ctx.rows4, images.data_ptr(), gptr, temp.data_ptr(),
                   g_l1.data_ptr(), g_ssim.data_ptr(), d_images.data_ptr(), _stream())
-        return d_images, None, None, None
+        return d_images, None, None, None, None
 
 
-def fused_l1_ssim_batched(images, gts_u8, rows4, *, deterministic=None):
+def fused_l1_ssim_batched(images, gts_u8, rows4, *, deterministic=None, gt_full=False):
     """The strip losses of the B cameras of a batch in one launch.  images (B,3,H,W); gts_u8: list of B CUDA uint8
     strips (3,rows,W) (None where rows == 0); rows4: B tuples (row0, row1, count_row0, count_row1).
     -> (B,2) = (Ll1, ssim_loss) per camera, both normalised by 3*H*W; zeros for cameras without rows.
     deterministic: None follows torch.use_deterministic_algorithms; when on, the per-CTA partial sums are added in a fixed
-    order (gs_loss_forward_batched_det), the same bits on every run."""
+    order (gs_loss_forward_batched_det), the same bits on every run.
+    gt_full: gts_u8 are the views' whole (3,H,W) images, read in place at rows [row0, row1) (gs_loss_*_batched_gt_full):
+    the same bits as passing the strips gt[:, row0:row1, :], without copying them out."""
     return _FusedL1SSIMBatched.apply(images, list(gts_u8), [tuple(int(v) for v in r) for r in rows4],
-                                     deterministic_enabled(deterministic))
+                                     deterministic_enabled(deterministic), bool(gt_full))
 
 
 def get_local2j_ids_bool(image_height, image_width, rank, world_size, means2D, radii, dist_global_strategy,
@@ -810,27 +815,36 @@ class _FusedLoss(torch.autograd.Function):
     product with a cached weight vector, and the backward hands (g (1 - lambda), -g lambda) to gs_loss_backward."""
 
     @staticmethod
-    def forward(ctx, image, gt_u8, row0, row1, crow0, crow1, lambda_dssim, det):
+    def forward(ctx, image, gt_u8, row0, row1, crow0, crow1, lambda_dssim, det, gt_full):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         image = _f32c(image, "image")
+        what = "image (3, H, W)" if gt_full else "strip (3, rows, W)"
         if gt_u8.dtype != torch.uint8 or not gt_u8.is_cuda:
-            raise TypeError("gt strip must be a CUDA uint8 tensor (3, rows, W)")
+            raise TypeError(f"gt {what} must be a CUDA uint8 tensor")
         gt_u8 = gt_u8.contiguous()
         _, H, W = image.shape
         rows = row1 - row0
-        if tuple(gt_u8.shape) != (3, rows, W):
-            raise ValueError(f"gt strip must be (3,{rows},{W}), got {tuple(gt_u8.shape)}")
+        want = (3, H, W) if gt_full else (3, rows, W)
+        if tuple(gt_u8.shape) != want:
+            raise ValueError(f"gt {what} must be {want}, got {tuple(gt_u8.shape)}")
         key = (image.device, float(lambda_dssim))
         if key not in _LOSS_W:
             _LOSS_W[key] = torch.tensor([1.0 - lambda_dssim, -lambda_dssim], dtype=torch.float32, device=image.device)
         w = _LOSS_W[key]
         sfx = "_det" if det else ""
-        tb = _lib.query("gs_loss_temp_bytes" + sfx, rows, W)
-        temp = torch.empty((tb,), dtype=torch.uint8, device=image.device)
         out = torch.empty((2,), dtype=torch.float32, device=image.device)
-        _lib.call("gs_loss_forward" + sfx, H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
-                  out.data_ptr(), temp.data_ptr(), tb, _stream())
-        ctx.rows, ctx.w = (row0, row1, crow0, crow1), w
+        if gt_full:   # the one-view batch of the in-place entry points: the same kernel, the same bits
+            rows4 = _i32_array([row0, row1, crow0, crow1])
+            tb = _lib.query("gs_loss_temp_bytes_batched" + sfx, 1, rows4, W)
+            temp = torch.empty((tb,), dtype=torch.uint8, device=image.device)
+            _lib.call("gs_loss_forward_batched_gt_full" + sfx, 1, H, W, rows4, image.data_ptr(),
+                      (C.c_void_p * 1)(gt_u8.data_ptr()), out.data_ptr(), temp.data_ptr(), tb, _stream())
+        else:
+            tb = _lib.query("gs_loss_temp_bytes" + sfx, rows, W)
+            temp = torch.empty((tb,), dtype=torch.uint8, device=image.device)
+            _lib.call("gs_loss_forward" + sfx, H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
+                      out.data_ptr(), temp.data_ptr(), tb, _stream())
+        ctx.rows, ctx.w, ctx.gt_full = (row0, row1, crow0, crow1), w, gt_full
         ctx.save_for_backward(image, gt_u8, temp)
         return torch.dot(out, w) + float(lambda_dssim)
 
@@ -840,21 +854,28 @@ class _FusedLoss(torch.autograd.Function):
         _, H, W = image.shape
         row0, row1, crow0, crow1 = ctx.rows
         if g is None:
-            return None, None, None, None, None, None, None, None
+            return None, None, None, None, None, None, None, None, None
         gw = (g.to(torch.float32) * ctx.w).contiguous()      # (g (1 - lambda), -g lambda)
         d_image = torch.empty_like(image)
-        _lib.call("gs_loss_backward", H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
-                  temp.data_ptr(), gw.data_ptr(), gw.data_ptr() + 4, d_image.data_ptr(), _stream())
-        return d_image, None, None, None, None, None, None, None
+        if ctx.gt_full:
+            _lib.call("gs_loss_backward_batched_gt_full", 1, H, W, _i32_array(ctx.rows), image.data_ptr(),
+                      (C.c_void_p * 1)(gt_u8.data_ptr()), temp.data_ptr(), gw.data_ptr(), gw.data_ptr() + 4,
+                      d_image.data_ptr(), _stream())
+        else:
+            _lib.call("gs_loss_backward", H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
+                      temp.data_ptr(), gw.data_ptr(), gw.data_ptr() + 4, d_image.data_ptr(), _stream())
+        return d_image, None, None, None, None, None, None, None, None
 
 
-def fused_loss(image, gt_u8, row0, row1, lambda_dssim, count_row0=None, count_row1=None, *, deterministic=None):
+def fused_loss(image, gt_u8, row0, row1, lambda_dssim, count_row0=None, count_row1=None, *, deterministic=None,
+               gt_full=False):
     """-> 0-dim loss (1 - lambda) Ll1 + lambda (1 - ssim) of the strip rows [row0, row1) (same window / count-row
-    semantics as fused_l1_ssim; deterministic as in fused_l1_ssim_batched)."""
+    semantics as fused_l1_ssim; deterministic as in fused_l1_ssim_batched).  gt_full: gt_u8 is the whole (3,H,W) image,
+    read in place (as in fused_l1_ssim_batched)."""
     c0 = int(row0) if count_row0 is None else int(count_row0)
     c1 = int(row1) if count_row1 is None else int(count_row1)
     return _FusedLoss.apply(image, gt_u8, int(row0), int(row1), c0, c1, float(lambda_dssim),
-                            deterministic_enabled(deterministic))
+                            deterministic_enabled(deterministic), bool(gt_full))
 
 
 # ---------------------------------------------------------------------------------------------------------

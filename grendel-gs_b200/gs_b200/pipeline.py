@@ -11,6 +11,8 @@ with the same partitioning rules:
     (gaussian_renderer/__init__.py:542-698).
 """
 
+import operator
+
 import torch
 import torch.nn as nn
 
@@ -127,7 +129,9 @@ class Trainer:
                  fused_activations=True, border_exchange=False, batched_render=True, peer_exchange=None,
                  peer_cap_rows=None, shard=None, load_balance=True, heuristic_decay=0.0,
                  distributed_dataset_storage=False, feedback_lag=None, max_sh_degree=3, deterministic=False):
-        """scene: the WHOLE scene (sliced here into this rank's contiguous shard), or -- shard=(lo, hi, n_total) -- only
+        """cams, gts_pinned: the camera set -- N cameras and their uint8 (3,H,W) host images, all of one size (the reference
+        keeps one global TILE_Y); each step trains on the views it lists (step(views=...)), all N by default.
+        scene: the WHOLE scene (sliced here into this rank's contiguous shard), or -- shard=(lo, hi, n_total) -- only
         this rank's Gaussians [lo, hi) of an n_total-Gaussian scene (synthetic.make_scene_shard).
         load_balance: feed the measured render times back into the strip division after every step
         (finish_strategy_final, workload_division.py:944-998; only where the reference's gate enables it).
@@ -202,33 +206,39 @@ class Trainer:
         self.iteration = 0
         self.balance_log = []      # (iteration, division rows of camera 0) whenever the division moved
         self.dcams = [DeviceCamera(c, device) for c in cams]
+        if not self.dcams:
+            raise ValueError("a Trainer needs at least one camera")
         self.H, self.W = self.dcams[0].image_height, self.dcams[0].image_width
+        sizes = {(c.image_height, c.image_width) for c in self.dcams}
+        if gts_pinned is not None:
+            if len(gts_pinned) != len(self.dcams):
+                raise ValueError(f"{len(self.dcams)} cameras but {len(gts_pinned)} ground-truth images")
+            sizes |= {(int(g.shape[-2]), int(g.shape[-1])) for g in gts_pinned}
+        if len(sizes) > 1:
+            raise ValueError(f"all cameras and images of a Trainer must share one image size (one TILE_Y, as in the "
+                             f"reference); got (H, W) = {sorted(sizes)}")
         self.tile_y, self.tile_x = (self.H + 15) // 16, (self.W + 15) // 16
         self.distributed_dataset_storage = bool(distributed_dataset_storage) and world > 1
         self.gts_host = gts_pinned                      # uint8 (3,H,W) pinned host tensors
-        # copies for the "inputs resident" leg (not needed by ranks without pixels in distributed-storage mode)
+        # the "inputs resident" leg keeps every image on the device (--preload_dataset_to_gpu, scene/cameras.py:67-68); its
+        # loss reads the strip rows in place (ops.fused_l1_ssim_batched(gt_full=True)).  Not needed by ranks without
+        # pixels in distributed-storage mode.
         self.gts_dev = [g.to(device) for g in gts_pinned] if gts_pinned is not None else None
         self.history = StrategyHistory([c.uid for c in self.dcams], self.tile_y, world)
-        self._strip_cache = {}
-        self._cams_packed = None   # (B,40) camera table of the batched preprocess (cameras are fixed per Trainer)
-        self._strategy_cache = None
+        self._strip_cache = {}     # pinned copies of the strips of non-pinned host images (resident=False)
+        # (N,40) host table of the batched preprocess: a step copies the rows of its views to the device
+        self._cam_rows = ops.pack_cameras([c.settings() for c in self.dcams]).cpu()
+        self._cams_dev = None      # (views, (B,40) device table) of the last step
+        self._strategy_cache = None   # ((history version, the batch's camera uids), strategies)
         self._mask_cache = {}
         self._bmask_cache = {}
         self._n_renders = 0
         self._copy_stream = None
-        self._loss_host = torch.zeros((1,), dtype=torch.float32).pin_memory()
+        self._loss_host = None
         self._info = {}
         self._h2d = 0
 
     # -- ground truth strips (load_camera_from_cpu_to_all_gpu, loss_distribution.py:2395-2533) ------------
-    def _gt_strip(self, k, y0, y1, resident):
-        key = (k, y0, y1, resident)
-        if resident:
-            if key not in self._strip_cache:
-                self._strip_cache[key] = self.gts_dev[k][:, y0:y1, :].contiguous()
-            return self._strip_cache[key]
-        return self._strip_h2d(k, y0, y1)
-
     def _strip_h2d(self, k, y0, y1):
         """Rows [y0, y1) of the pinned (3,H,W) uint8 ground truth -> a (3, rows, W) device strip: the rows of one channel
         are contiguous in the pinned image, so the strip is three asynchronous copies straight out of it -- no staging
@@ -258,16 +268,59 @@ class Trainer:
         self.trace[name] = self.trace.get(name, 0.0) + (now - self._t_last) * 1e3
         self._t_last = now
 
-    def step(self, resident=True):
-        """One forward + loss + backward over the batch.  resident=False copies the GT strips from pinned host
-        memory inside the step and reads the loss back (the end-to-end leg); returns the loss as a float then."""
+    def step(self, views=None, resident=True):
+        """One forward + loss + backward over a batch of the camera set.  views: indices into the cameras, in batch
+        order (a camera may appear more than once); None = all cameras in order.  The caller chooses them (the reference
+        draws --bsz per step, train_internal.py:134).  resident=False copies the GT strips from pinned host memory inside
+        the step and reads the loss back (the end-to-end leg); returns the loss as a float then."""
+        views = self._batch_views(views)
         ops.STEP_STREAM = torch.cuda.current_stream().cuda_stream   # every kernel of the step goes to this stream
         try:
-            return self._step(resident)
+            return self._step(views, resident)
         finally:
             ops.STEP_STREAM = None
 
-    def _step(self, resident):
+    def _batch_views(self, views):
+        N = len(self.dcams)
+        if views is None:
+            return tuple(range(N))
+        views = tuple(operator.index(v) for v in views)   # TypeError for anything but integers
+        if not 1 <= len(views) <= 64:   # GS_MAX_VIEWS of the batched kernels
+            raise ValueError(f"a step trains on 1 to 64 views, got {len(views)}")
+        for v in views:
+            if not 0 <= v < N:
+                raise ValueError(f"view {v} is not a camera of this Trainer (0..{N - 1})")
+        return views
+
+    def _batch_strategies(self, uids):
+        """The strip division of a batch, cached per (history version, the batch's camera uids): it follows the cost
+        heuristics of exactly those cameras.  The division-keyed mask / strip caches are only dropped when the load
+        balancer moved the strips (a new history version), so batches that come and go keep theirs."""
+        ver = len(self.history.history)   # the division only changes when the cost heuristic is updated
+        prev = self._strategy_cache
+        if prev is not None and prev[0] == (ver, uids):
+            return prev[1]
+        new = start_strategy(list(uids), self.history, self.world, self.rank)[0]
+        moved = prev is None or len(new) != len(prev[1]) or any(
+            a.gpu_ids != b.gpu_ids or a.division_pos != b.division_pos for a, b in zip(new, prev[1]))
+        self._strategy_cache = ((ver, uids), new)
+        if moved and (prev is None or prev[0][0] != ver):   # per-division caches belong to the old boundaries
+            self._strip_cache.clear(); self._mask_cache.clear(); self._bmask_cache.clear()
+            self.balance_log.append((self.iteration, [list(st.division_pos) for st in new],
+                                     [list(st.gpu_ids) for st in new]))
+        return new
+
+    def _camera_table(self, views):
+        """(B,40) device camera table of the batched preprocess: the views' rows gathered into pinned host memory and
+        copied asynchronously (no host sync; the pinned block is not reused before the copy has run).  Kept while the
+        views stay the same."""
+        if self._cams_dev is None or self._cams_dev[0] != views:
+            stage = torch.empty((len(views), self._cam_rows.shape[1]), dtype=torch.float32, pin_memory=True)
+            torch.index_select(self._cam_rows, 0, torch.tensor(views, dtype=torch.int64), out=stage)
+            self._cams_dev = (views, stage.to(self.device, non_blocking=True))
+        return self._cams_dev[1]
+
+    def _step(self, views, resident):
         import os as _os, time as _time
         self._trace_on = _os.environ.get("GS_B200_TRACE") == "1"
         self._ex.TRACE = self._mark if self._trace_on else None
@@ -282,28 +335,19 @@ class Trainer:
             t.grad = None
         self._h2d = 0
         ops.LAST_R_TOTAL = 0
-        uids = [c.uid for c in self.dcams]
-        ver = len(self.history.history)   # the division only changes when the cost heuristic is updated
-        if self._strategy_cache is None or self._strategy_cache[0] != ver:
-            new = start_strategy(uids, self.history, self.world, self.rank)[0]
-            moved = self._strategy_cache is None or any(
-                a.gpu_ids != b.gpu_ids or a.division_pos != b.division_pos for a, b in zip(new, self._strategy_cache[1]))
-            self._strategy_cache = (ver, new)
-            if moved:   # per-division caches (masks, pinned GT strips) belong to the old boundaries
-                self._strip_cache.clear(); self._mask_cache.clear(); self._bmask_cache.clear()
-                self.balance_log.append((self.iteration, [list(st.division_pos) for st in new],
-                                         [list(st.gpu_ids) for st in new]))
-        strategies = self._strategy_cache[1]
+        dcams = [self.dcams[i] for i in views]
+        strategies = self._batch_strategies(tuple(c.uid for c in dcams))
         self._tasks = [[(k, st.division_pos[st.gpu_ids.index(g)], st.division_pos[st.gpu_ids.index(g) + 1])
                         for k, st in enumerate(strategies) if g in st.gpu_ids] for g in range(self.world)]
-        settings = [c.settings(p.active_sh_degree) for c in self.dcams]
+        settings = [c.settings(p.active_sh_degree) for c in dcams]
         # "Asynchronously load ground-truth image to GPU" (loss_distribution.py:2399): the strips this rank needs are
         # copied from pinned host memory on a side stream while preprocess / binning / blend run, and the loss waits
         # on the copy's event.
         gt_ready = {}
         if not resident and self.distributed_dataset_storage:
             from . import gt_scatter
-            strips, h2d = gt_scatter.scatter_gt_strips(self.gts_host if self.rank == 0 else self.W, self._tasks, self.H,
+            batch_host = [self.gts_host[i] for i in views] if self.rank == 0 else self.W
+            strips, h2d = gt_scatter.scatter_gt_strips(batch_host, self._tasks, self.H,
                                                        self.device, self.rank, self.world, self.group)
             self._h2d += h2d
             ev = torch.cuda.Event()
@@ -317,22 +361,20 @@ class Trainer:
                 if rows is None:
                     continue
                 with torch.cuda.stream(self._copy_stream):
-                    d = self._strip_h2d(k, rows[0], rows[1])
+                    d = self._strip_h2d(views[k], rows[0], rows[1])
                     ev = torch.cuda.Event()
                     ev.record(self._copy_stream)
                 gt_ready[k] = (d, ev)
         if not self.fused_activations:  # the reference's five activation kernels + cat (__init__.py:902-906)
             xyz, scaling, rotation, feats, opacity = p.get_xyz, p.get_scaling, p.get_rotation, p.get_features, p.get_opacity
-        collectors = [{} for _ in self.dcams]
+        collectors = [{} for _ in dcams]
         screen = []
         B = len(settings)
         use_batched = self.batched_render and B > 1 and not self.border_exchange
         if self.fused_activations and len(settings) > 1:
             # all B cameras in ONE launch: every Gaussian is read once and projected into each camera
-            if self._cams_packed is None:
-                self._cams_packed = ops_.pack_cameras(settings)
             bm2, brgb, bco, bradii, bdepths = ops_.preprocess_gaussians_batched(
-                p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation, p._opacity, self._cams_packed,
+                p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation, p._opacity, self._camera_table(views),
                 self.W, self.H, p.active_sh_degree)
             bm2.retain_grad()   # (B,P,2): densification reads bm2.grad[k] (means2D.grad of camera k, densification.py:24)
             batched = (bm2, brgb, bco, bradii, bdepths)
@@ -408,14 +450,14 @@ class Trainer:
             for k, (y0, y1, _c0, _c1) in enumerate(rows4):
                 if y1 == y0:
                     gts.append(None)
-                elif resident:
-                    gts.append(self._gt_strip(k, y0, y1, True))
+                elif resident:   # the whole resident image, read in place
+                    gts.append(self.gts_dev[views[k]])
                 else:
                     gt, ev = gt_ready[k]
                     torch.cuda.current_stream().wait_event(ev)
                     gt.record_stream(torch.cuda.current_stream())
                     gts.append(gt)
-            l1_ssim = ops_.fused_l1_ssim_batched(images, gts, rows4, deterministic=self.deterministic)
+            l1_ssim = ops_.fused_l1_ssim_batched(images, gts, rows4, deterministic=self.deterministic, gt_full=resident)
             # sum over the local strips of (1 - lambda) Ll1 + lambda (1 - ssim)
             loss_sum = torch.dot(l1_ssim.reshape(-1), coef) + const
             Vp = int(view_start[-1])
@@ -439,16 +481,19 @@ class Trainer:
             if self.border_exchange and self.world > 1 and len(st.gpu_ids) > 1:
                 from . import border
                 image, (r0, r1), _ = border.add_remote_border_rows(image, st, self.H, self.group)
-                loss = ops_.fused_loss(image, self.gts_dev[k][:, r0:r1, :].contiguous(), r0, r1, self.lambda_dssim, y0, y1,
-                                       deterministic=self.deterministic)
+                loss = ops_.fused_loss(image, self.gts_dev[views[k]], r0, r1, self.lambda_dssim, y0, y1,
+                                       deterministic=self.deterministic, gt_full=True)
             else:
                 if resident:
-                    gt = self._gt_strip(k, y0, y1, True)
+                    gt = self.gts_dev[views[k]]
                 else:
                     gt, ev = gt_ready[k]
                     torch.cuda.current_stream().wait_event(ev)
                     gt.record_stream(torch.cuda.current_stream())
-                loss = ops_.fused_loss(image, gt, y0, y1, self.lambda_dssim, deterministic=self.deterministic)
+                # a strip of every row is the resident image itself: the strip form reads it with no host-side row
+                # tables (the single-rank step); only a part of the image needs the in-place form
+                loss = ops_.fused_loss(image, gt, y0, y1, self.lambda_dssim, deterministic=self.deterministic,
+                                       gt_full=resident and (y0, y1) != (0, self.H))
             loss_sum = loss if loss_sum is None else loss_sum + loss
             Vp += m2.shape[0]
             Pl += (y1 - y0) * self.W
@@ -462,6 +507,8 @@ class Trainer:
         self._mark("t time feedback")
         if resident:
             return None
+        if self._loss_host is None:
+            self._loss_host = torch.zeros((1,), dtype=torch.float32).pin_memory()
         self._loss_host.copy_(loss_sum.detach().reshape(1), non_blocking=True)
         torch.cuda.current_stream().synchronize()
         return float(self._loss_host[0])

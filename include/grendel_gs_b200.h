@@ -433,6 +433,22 @@ GS_API int gs_loss_forward_batched_det(int num_views, int image_height, int imag
                                        const float *image, const void *const *gt_u8_ptrs_host, float *out_l1_ssim,
                                        void *temp, size_t temp_bytes, void *stream);
 
+/* The batched loss with each view's ground truth as its WHOLE (3,H,W) uint8 image (the training images kept resident on
+ * the device, --preload_dataset_to_gpu, scene/cameras.py:67-68), read in place at rows [row0,row1) with channel pitch H*W:
+ * no strip is copied out of it.  gt_u8_ptrs_host[v] must be 16-byte aligned (the start of the image).  Same arguments,
+ * temp sizes (gs_loss_temp_bytes_batched / _det) and results, bit for bit, as the strip forms given the strips
+ * image[:, row0:row1, :]. */
+GS_API int gs_loss_forward_batched_gt_full(int num_views, int image_height, int image_width, const int32_t *rows4_host,
+                                           const float *image, const void *const *gt_u8_ptrs_host, float *out_l1_ssim,
+                                           void *temp, size_t temp_bytes, void *stream);
+GS_API int gs_loss_forward_batched_gt_full_det(int num_views, int image_height, int image_width,
+                                               const int32_t *rows4_host, const float *image,
+                                               const void *const *gt_u8_ptrs_host, float *out_l1_ssim, void *temp,
+                                               size_t temp_bytes, void *stream);
+GS_API int gs_loss_backward_batched_gt_full(int num_views, int image_height, int image_width, const int32_t *rows4_host,
+                                            const float *image, const void *const *gt_u8_ptrs_host, const void *temp,
+                                            const float *grad_l1, const float *grad_ssim, float *dL_dimage, void *stream);
+
 /* ---- all-to-all staging -- gaussian_renderer/__init__.py:590-607,651-658 --------------------------
  * Replaces the per-(destination, camera) nonzero() + index_select + torch.cat glue around the sparse
  * all-to-all: rows of 11 floats forward (means2D 2, rgb 3, conic_opacity 4, radius as float, depth), 9 floats
