@@ -370,28 +370,42 @@ def _grad_block(P, dev):
 
 
 class _RenderGaussians(torch.autograd.Function):
+    """The B cameras of a batch in ONE pass (gs_render_*_batched): the splats of all cameras concatenated (camera k = rows
+    [view_start[k], view_start[k+1])), masks (B,T), images (B,3,H,W).  view_start None: render_gaussians' one camera,
+    view_start = [0, P], whose outputs are allocated without the view axis."""
+
     @staticmethod
-    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, rs, collector, want_ts, log, det):
+    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, view_start, rs, collector, want_ts, log,
+                det):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         means2D, conic_opacity, rgb = _f32c(means2D, "means2D"), _f32c(conic_opacity, "conic_opacity"), _f32c(rgb, "rgb")
         depths = _f32c(depths, "depths")
         if radii.dtype != torch.int32:
             radii = radii.to(torch.int32)
         radii = radii.contiguous()
-        P = means2D.shape[0]
+        single = view_start is None
+        if single:
+            view_start = [0, means2D.shape[0]]
+        B = len(view_start) - 1
+        P = int(view_start[B])
+        if not 1 <= B <= MAX_VIEWS:
+            raise ValueError(f"1..{MAX_VIEWS} views per batched render, got {B}")
+        if means2D.shape[0] != P:
+            raise ValueError(f"view_start ends at {P} but {means2D.shape[0]} splats were passed")
         H, W = int(rs.image_height), int(rs.image_width)
         ty, tx = _tiles(rs)
         T = ty * tx
         dev = means2D.device
         if compute_locally is None:
-            cl = torch.ones((T,), dtype=torch.uint8, device=dev)
+            cl = torch.ones((B * T,), dtype=torch.uint8, device=dev)
         else:
-            if compute_locally.numel() != T:
-                raise ValueError(f"compute_locally must have {ty}x{tx} entries, got {tuple(compute_locally.shape)}")
+            if compute_locally.numel() != B * T:
+                raise ValueError(f"compute_locally must have {B}x{ty}x{tx} entries, got {tuple(compute_locally.shape)}")
             cl = compute_locally.contiguous()
             cl = cl.view(torch.uint8) if cl.dtype == torch.bool else cl.to(torch.uint8)
         bg = _f32c(rs.bg, "bg")
         s = _stream()
+        vs = _i32_array(view_start)
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
         Pq = _q(P)
@@ -400,84 +414,85 @@ class _RenderGaussians(torch.autograd.Function):
         rec = torch.empty((Pq, 12), dtype=torch.float32, device=dev)
         tb = _lib.query("gs_render_count_temp_bytes", Pq)
         temp = torch.empty((tb,), dtype=torch.uint8, device=dev)
-        ranges = torch.empty((T, 2), dtype=torch.int32, device=dev)
-        image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-        final_T = torch.empty((H, W), dtype=torch.float32, device=dev)
-        n_contrib = torch.empty((H, W), dtype=torch.int32, device=dev)
-        stats = torch.empty((3,), dtype=torch.int64, device=dev)
+        ranges = torch.empty((B * T, 2), dtype=torch.int32, device=dev)
+        lead = () if single else (B,)
+        image = torch.empty((*lead, 3, H, W), dtype=torch.float32, device=dev)
+        final_T = torch.empty((B, H, W), dtype=torch.float32, device=dev)
+        n_contrib = torch.empty((B, H, W), dtype=torch.int32, device=dev)
+        stats = torch.empty((*lead, 3), dtype=torch.int64, device=dev)
         log_tiles = log is not None and log.debug
-        ts = torch.empty((ty, tx, 3), dtype=torch.int64, device=dev) if want_ts or log_tiles else None
+        ts = torch.empty((*lead, ty, tx, 3), dtype=torch.int64, device=dev) if want_ts or log_tiles else None
         needs_grad = means2D.requires_grad or conic_opacity.requires_grad or rgb.requires_grad
         det = det and needs_grad    # a forward-only render is the same bits either way
         with _gpu_time(log, "render forward"):   # the count, the sort and the blend of this call (stages 24-70)
             R = C.c_int64(0)
             ticket = C.c_void_p()
-            _lib.call("gs_render_count_launch", 1, None, P, H, W, means2D.data_ptr(), conic_opacity.data_ptr(), rgb.data_ptr(),
-                      depths.data_ptr(), radii.data_ptr(), cl.data_ptr(), order.data_ptr(), offsets.data_ptr(),
-                      rec.data_ptr(), temp.data_ptr(), tb, C.byref(ticket), s)
+            _lib.call("gs_render_count_launch", B, vs, P, H, W, means2D.data_ptr(), conic_opacity.data_ptr(),
+                      rgb.data_ptr(), depths.data_ptr(), radii.data_ptr(), cl.data_ptr(), order.data_ptr(),
+                      offsets.data_ptr(), rec.data_ptr(), temp.data_ptr(), tb, C.byref(ticket), s)
             # not P: the splat count of a strip varies from step to step, R follows it smoothly
-            key = (1, H, W, needs_grad) if not det else (1, H, W, needs_grad, "det")
-            pre = _instance_buffers_before_sync(key, T, dev, needs_grad, det)    # host work while the count / sort / scan run
+            key = (B, H, W, needs_grad) if not det else (B, H, W, needs_grad, "det")
+            pre = _instance_buffers_before_sync(key, B * T, dev, needs_grad, det)   # host work while the count / sort / scan run
             _lib.call("gs_render_count_read", ticket, C.byref(R), s)   # the operator's one host sync
             R = int(R.value)
             global LAST_R_TOTAL
             LAST_R_TOTAL += R
-            ib = _instance_buffers_after_sync(key, pre, R, T, dev, needs_grad, det)
+            ib = _instance_buffers_after_sync(key, pre, R, B * T, dev, needs_grad, det)
             seg = ib.seg if R > 0 else None
             if det:
-                _lib.call("gs_render_forward_det", 1, None, P, R, H, W, means2D.data_ptr(), radii.data_ptr(),
-                          cl.data_ptr(), order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(),
-                          ib.row(ib.tiles, 0), ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1),
-                          ib.sorted_u.data_ptr(), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(), image.data_ptr(),
-                          final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts), _lib.ptr(seg),
+                _lib.call("gs_render_forward_det", B, vs, P, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
+                          order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
+                          ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sorted_u.data_ptr(),
+                          ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(), image.data_ptr(), final_T.data_ptr(),
+                          n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts), _lib.ptr(seg),
                           ib.segb if seg is not None else 0, s)
             else:
-                _lib.call("gs_render_forward_ts", P, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
-                          order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
-                          ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(),
-                          image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts),
-                          _lib.ptr(seg), ib.segb if seg is not None else 0, s)
+                _lib.call("gs_render_forward_batched_ts", B, vs, R, H, W, means2D.data_ptr(), radii.data_ptr(),
+                          cl.data_ptr(), order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(),
+                          ib.row(ib.tiles, 0), ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1),
+                          ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(), image.data_ptr(), final_T.data_ptr(),
+                          n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts), _lib.ptr(seg),
+                          ib.segb if seg is not None else 0, s)
             ev1.record()
         if log_tiles:
             statlog.append(log.path("n_contrib"), statlog.n_contrib_text(
                 log.iteration, log.local_rank, log.world_size, H, W, cl.cpu(), ranges.cpu(), ts.cpu()))
         _timed(collector, "forward_render_time", ev0, ev1)
         ids_sorted = ib.ids[1]    # a view: the (tile, id) scratch stays alive until the backward has run (16 B / instance)
-        ctx.rs, ctx.R, ctx.P, ctx.collector, ctx.seg, ctx.log = rs, R, P, collector, seg, log
+        ctx.rs, ctx.R, ctx.P, ctx.B, ctx.collector, ctx.seg, ctx.log = rs, R, P, B, collector, seg, log
         # deterministic backward: the depth order and offsets of the count, the slots of the sort and the row workspace
         ctx.det = (order, offsets, ib.sorted_u, _det_workspace(ib, Pq, dev)) if det else None
         ctx.save_for_backward(rec, bg, cl, ranges, ids_sorted, final_T, n_contrib)
-        n_render, n_consider, n_contrib_sum = stats[0], stats[1], stats[2]
+        outs = (stats[0], stats[1], stats[2]) if single else (stats,)   # n_render, n_consider, n_contrib
         if want_ts:
-            ctx.mark_non_differentiable(n_render, n_consider, n_contrib_sum, ts)
-            return image, n_render, n_consider, n_contrib_sum, ts
-        ctx.mark_non_differentiable(n_render, n_consider, n_contrib_sum)
-        return image, n_render, n_consider, n_contrib_sum
+            outs += (ts,)
+        ctx.mark_non_differentiable(*outs)
+        return (image, *outs)
 
     @staticmethod
     def backward(ctx, g_image, *_unused):
         rec, bg, cl, ranges, ids_sorted, final_T, n_contrib = ctx.saved_tensors
-        rs, R, P = ctx.rs, ctx.R, ctx.P
+        rs, R, P, B = ctx.rs, ctx.R, ctx.P, ctx.B
         H, W = int(rs.image_height), int(rs.image_width)
         dev = rec.device
-        g_image = torch.zeros((3, H, W), dtype=torch.float32, device=dev) if g_image is None else _f32c(g_image, "grad")
+        g_image = torch.zeros((B, 3, H, W), dtype=torch.float32, device=dev) if g_image is None else _f32c(g_image, "grad")
         d_means2D, d_conic, d_rgb = _grad_block(P, dev)
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
         seg = ctx.seg
         with _gpu_time(ctx.log, "render backward"):
             if ctx.det is not None:
-                _render_backward_det(ctx.det, 1, P, R, H, W, rec, bg, cl, ranges, ids_sorted, final_T, n_contrib,
+                _render_backward_det(ctx.det, B, P, R, H, W, rec, bg, cl, ranges, ids_sorted, final_T, n_contrib,
                                      g_image, seg, d_means2D, d_conic, d_rgb)
             else:
-                _lib.call("gs_render_backward", P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(), ranges.data_ptr(),
-                          ids_sorted.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), g_image.data_ptr(),
-                          _lib.ptr(seg), 0 if seg is None else seg.numel(),
+                _lib.call("gs_render_backward_batched", B, P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(),
+                          ranges.data_ptr(), ids_sorted.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(),
+                          g_image.data_ptr(), _lib.ptr(seg), 0 if seg is None else seg.numel(),
                           d_means2D.data_ptr(), d_conic.data_ptr(), d_rgb.data_ptr(), _stream())
         ctx.seg = ctx.det = None
         ev1.record()
         _timed(ctx.collector, "backward_render_time", ev0, ev1)
-        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None, None, None
+        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None, None, None, None
 
 
 def _render_backward_det(det, B, P, R, H, W, rec, bg, cl, ranges, ids_sorted, final_T, n_contrib, g_image, seg, d_means2D,
@@ -520,8 +535,9 @@ def render_gaussians(means2D, conic_opacity, rgb, depths, radii, compute_locally
     collector = None
     if isinstance(cuda_args, dict):
         collector = cuda_args.setdefault("stats_collector", {})
-    return _RenderGaussians.apply(means2D, conic_opacity, rgb, depths, radii, compute_locally, raster_settings, collector,
-                                  bool(tile_stats), statlog.request(cuda_args), deterministic_enabled(deterministic))
+    return _RenderGaussians.apply(means2D, conic_opacity, rgb, depths, radii, compute_locally, None, raster_settings,
+                                  collector, bool(tile_stats), statlog.request(cuda_args),
+                                  deterministic_enabled(deterministic))
 
 
 MAX_VIEWS = 64   # GS_MAX_VIEWS
@@ -529,117 +545,6 @@ MAX_VIEWS = 64   # GS_MAX_VIEWS
 
 def _i32_array(vals):
     return (C.c_int32 * len(vals))(*[int(v) for v in vals])
-
-
-class _RenderGaussiansBatched(torch.autograd.Function):
-    """render_gaussians for the B cameras of a batch in ONE pass (gs_render_*_batched): the splats of all cameras
-    concatenated (camera k = rows [view_start[k], view_start[k+1])), masks (B,T), images (B,3,H,W)."""
-
-    @staticmethod
-    def forward(ctx, means2D, conic_opacity, rgb, depths, radii, compute_locally, view_start, rs, collector, want_ts, det):
-        ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
-        means2D, conic_opacity, rgb = _f32c(means2D, "means2D"), _f32c(conic_opacity, "conic_opacity"), _f32c(rgb, "rgb")
-        depths = _f32c(depths, "depths")
-        if radii.dtype != torch.int32:
-            radii = radii.to(torch.int32)
-        radii = radii.contiguous()
-        B = len(view_start) - 1
-        P = int(view_start[B])
-        if not 1 <= B <= MAX_VIEWS:
-            raise ValueError(f"1..{MAX_VIEWS} views per batched render, got {B}")
-        if means2D.shape[0] != P:
-            raise ValueError(f"view_start ends at {P} but {means2D.shape[0]} splats were passed")
-        H, W = int(rs.image_height), int(rs.image_width)
-        ty, tx = _tiles(rs)
-        T = ty * tx
-        dev = means2D.device
-        if compute_locally is None:
-            cl = torch.ones((B * T,), dtype=torch.uint8, device=dev)
-        else:
-            if compute_locally.numel() != B * T:
-                raise ValueError(f"compute_locally must have {B}x{ty}x{tx} entries, got {tuple(compute_locally.shape)}")
-            cl = compute_locally.contiguous()
-            cl = cl.view(torch.uint8) if cl.dtype == torch.bool else cl.to(torch.uint8)
-        bg = _f32c(rs.bg, "bg")
-        s = _stream()
-        vs = _i32_array(view_start)
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        ev0.record()
-        Pq = _q(P)
-        offsets = torch.empty((Pq,), dtype=torch.int32, device=dev)
-        order = torch.empty((Pq,), dtype=torch.int32, device=dev)
-        rec = torch.empty((Pq, 12), dtype=torch.float32, device=dev)
-        tb = _lib.query("gs_render_count_temp_bytes", Pq)
-        temp = torch.empty((tb,), dtype=torch.uint8, device=dev)
-        ranges = torch.empty((B * T, 2), dtype=torch.int32, device=dev)
-        image = torch.empty((B, 3, H, W), dtype=torch.float32, device=dev)
-        final_T = torch.empty((B, H, W), dtype=torch.float32, device=dev)
-        n_contrib = torch.empty((B, H, W), dtype=torch.int32, device=dev)
-        stats = torch.empty((B, 3), dtype=torch.int64, device=dev)
-        ts = torch.empty((B, ty, tx, 3), dtype=torch.int64, device=dev) if want_ts else None
-        needs_grad = means2D.requires_grad or conic_opacity.requires_grad or rgb.requires_grad
-        det = det and needs_grad    # a forward-only render is the same bits either way
-        R = C.c_int64(0)
-        ticket = C.c_void_p()
-        _lib.call("gs_render_count_launch", B, vs, P, H, W, means2D.data_ptr(), conic_opacity.data_ptr(), rgb.data_ptr(),
-                  depths.data_ptr(), radii.data_ptr(), cl.data_ptr(), order.data_ptr(), offsets.data_ptr(),
-                  rec.data_ptr(), temp.data_ptr(), tb, C.byref(ticket), s)
-        key = (B, H, W, needs_grad) if not det else (B, H, W, needs_grad, "det")
-        pre = _instance_buffers_before_sync(key, B * T, dev, needs_grad, det)   # host work while the count / sort / scan run
-        _lib.call("gs_render_count_read", ticket, C.byref(R), s)    # the operator's one host sync
-        R = int(R.value)
-        global LAST_R_TOTAL
-        LAST_R_TOTAL += R
-        ib = _instance_buffers_after_sync(key, pre, R, B * T, dev, needs_grad, det)
-        seg = ib.seg if R > 0 else None
-        if det:
-            _lib.call("gs_render_forward_det", B, vs, P, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
-                      order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
-                      ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sorted_u.data_ptr(),
-                      ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(), image.data_ptr(), final_T.data_ptr(),
-                      n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts), _lib.ptr(seg),
-                      ib.segb if seg is not None else 0, s)
-        else:
-            _lib.call("gs_render_forward_batched_ts", B, vs, R, H, W, means2D.data_ptr(), radii.data_ptr(), cl.data_ptr(),
-                      order.data_ptr(), offsets.data_ptr(), rec.data_ptr(), bg.data_ptr(), ib.row(ib.tiles, 0),
-                      ib.row(ib.ids, 0), ib.row(ib.tiles, 1), ib.row(ib.ids, 1), ib.sort_temp.data_ptr(), ib.sb, ranges.data_ptr(),
-                      image.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), stats.data_ptr(), _lib.ptr(ts),
-                      _lib.ptr(seg), ib.segb if seg is not None else 0, s)
-        ev1.record()
-        _timed(collector, "forward_render_time", ev0, ev1)
-        ids_sorted = ib.ids[1]    # a view: the (tile, id) scratch stays alive until the backward has run (16 B / instance)
-        ctx.rs, ctx.R, ctx.P, ctx.B, ctx.collector, ctx.seg = rs, R, P, B, collector, seg
-        ctx.det = (order, offsets, ib.sorted_u, _det_workspace(ib, Pq, dev)) if det else None
-        ctx.save_for_backward(rec, bg, cl, ranges, ids_sorted, final_T, n_contrib)
-        if want_ts:
-            ctx.mark_non_differentiable(stats, ts)
-            return image, stats, ts
-        ctx.mark_non_differentiable(stats)
-        return image, stats
-
-    @staticmethod
-    def backward(ctx, g_image, *_unused):
-        rec, bg, cl, ranges, ids_sorted, final_T, n_contrib = ctx.saved_tensors
-        rs, R, P, B = ctx.rs, ctx.R, ctx.P, ctx.B
-        H, W = int(rs.image_height), int(rs.image_width)
-        dev = rec.device
-        g_image = torch.zeros((B, 3, H, W), dtype=torch.float32, device=dev) if g_image is None else _f32c(g_image, "grad")
-        d_means2D, d_conic, d_rgb = _grad_block(P, dev)
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        ev0.record()
-        seg = ctx.seg
-        if ctx.det is not None:
-            _render_backward_det(ctx.det, B, P, R, H, W, rec, bg, cl, ranges, ids_sorted, final_T, n_contrib, g_image, seg,
-                                 d_means2D, d_conic, d_rgb)
-        else:
-            _lib.call("gs_render_backward_batched", B, P, R, H, W, rec.data_ptr(), bg.data_ptr(), cl.data_ptr(),
-                      ranges.data_ptr(), ids_sorted.data_ptr(), final_T.data_ptr(), n_contrib.data_ptr(), g_image.data_ptr(),
-                      _lib.ptr(seg), 0 if seg is None else seg.numel(),
-                      d_means2D.data_ptr(), d_conic.data_ptr(), d_rgb.data_ptr(), _stream())
-        ctx.seg = ctx.det = None
-        ev1.record()
-        _timed(ctx.collector, "backward_render_time", ev0, ev1)
-        return d_means2D, d_conic, d_rgb, None, None, None, None, None, None, None, None
 
 
 def render_gaussians_batched(means2D, conic_opacity, rgb, depths, radii, compute_locally, view_start, raster_settings,
@@ -654,24 +559,36 @@ def render_gaussians_batched(means2D, conic_opacity, rgb, depths, radii, compute
     collector = None
     if isinstance(cuda_args, dict):
         collector = cuda_args.setdefault("stats_collector", {})
-    return _RenderGaussiansBatched.apply(means2D, conic_opacity, rgb, depths, radii, compute_locally,
-                                         [int(v) for v in view_start], raster_settings, collector, bool(tile_stats),
-                                         deterministic_enabled(deterministic))
+    return _RenderGaussians.apply(means2D, conic_opacity, rgb, depths, radii, compute_locally,
+                                  [int(v) for v in view_start], raster_settings, collector, bool(tile_stats), None,
+                                  deterministic_enabled(deterministic))
 
 
-class _FusedL1SSIMBatched(torch.autograd.Function):
+_LOSS_W = {}
+
+
+class _FusedL1SSIM(torch.autograd.Function):
+    """Per-strip (Ll1, ssim) of loss_distribution.py:2536-2585 for the B views of `images` (B,3,H,W) in two kernels
+    instead of ~20 (gs_loss_*_batched[_gt_full][_det]).
+
+    single: the per-camera calls, `images` is the one view's (3,H,W) image; its ground truth is checked even without
+    rows, and the strip form refuses an empty window (gs_loss_forward's contract).  Without lambda_dssim the (B,2) sums
+    are returned, or for a single view the two 0-dim sums.  With it, one view's (1 - lambda) Ll1 + lambda (1 - ssim) is
+    ONE autograd node (train_internal.py:166-189 forms it with five elementwise kernels and as many in the backward): one
+    dot product with a cached weight vector, and the backward hands (g (1 - lambda), -g lambda) to the kernel."""
+
     @staticmethod
-    def forward(ctx, images, gts, rows4, det, gt_full):
+    def forward(ctx, images, gts, rows4, det, gt_full, single, lambda_dssim):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
         images = _f32c(images, "images")
-        B, _, H, W = images.shape
+        B, _, H, W = (1, *images.shape) if single else images.shape
         if len(gts) != B or len(rows4) != B:
             raise ValueError("one ground-truth strip and one (row0,row1,count_row0,count_row1) per view")
         what = "images (3, H, W)" if gt_full else "strips (3, rows, W)"
         keep = []
         for k, (gt, r) in enumerate(zip(gts, rows4)):
             rows = int(r[1]) - int(r[0])
-            if rows == 0:
+            if rows == 0 and not single:
                 keep.append(None)
                 continue
             if gt is None or gt.dtype != torch.uint8 or not gt.is_cuda:
@@ -680,32 +597,55 @@ class _FusedL1SSIMBatched(torch.autograd.Function):
             want = (3, H, W) if gt_full else (3, rows, W)
             if tuple(gt.shape) != want:
                 raise ValueError(f"gt {k} must be {want}, got {tuple(gt.shape)}")
+            if rows == 0 and not gt_full:   # a single view's strip form: gs_loss_forward refuses an empty strip
+                raise _lib.GsError(f"a strip needs rows: [{r[0]}, {r[1]}) is empty")
             keep.append(gt)
+        ctx.w = None
+        if lambda_dssim is not None:
+            key = (images.device, lambda_dssim)
+            if key not in _LOSS_W:
+                _LOSS_W[key] = torch.tensor([1.0 - lambda_dssim, -lambda_dssim], dtype=torch.float32, device=images.device)
+            ctx.w = _LOSS_W[key]
         flat = _i32_array([int(v) for r in rows4 for v in r])
         gptr = (C.c_void_p * B)(*[None if g is None else g.data_ptr() for g in keep])
         sfx = "_det" if det else ""
         tb = _lib.query("gs_loss_temp_bytes_batched" + sfx, B, flat, W)
         temp = torch.empty((tb,), dtype=torch.uint8, device=images.device)
-        out = torch.empty((B, 2), dtype=torch.float32, device=images.device)
+        out = torch.empty((2,) if single else (B, 2), dtype=torch.float32, device=images.device)
         full = "_gt_full" if gt_full else ""
         _lib.call("gs_loss_forward_batched" + full + sfx, B, H, W, flat, images.data_ptr(), gptr, out.data_ptr(),
                   temp.data_ptr(), tb, _stream())
-        ctx.rows4, ctx.gts, ctx.full = flat, keep, full
+        ctx.rows4, ctx.gts, ctx.full, ctx.pair = flat, keep, full, single and lambda_dssim is None
         ctx.save_for_backward(images, temp)
-        return out
+        if ctx.w is not None:
+            return torch.dot(out, ctx.w) + lambda_dssim
+        return (out[0], out[1]) if ctx.pair else out
 
     @staticmethod
-    def backward(ctx, g_out):
+    def backward(ctx, *g):
         images, temp = ctx.saved_tensors
-        B, _, H, W = images.shape
-        if g_out is None:
-            return None, None, None, None, None
-        g_l1, g_ssim = g_out[:, 0].to(torch.float32).contiguous(), g_out[:, 1].to(torch.float32).contiguous()
+        B, (H, W) = len(ctx.gts), images.shape[-2:]
+        if ctx.pair:
+            g_l1, g_ssim = (torch.zeros((), device=images.device) if x is None else x.to(torch.float32) for x in g)
+            p_l1, p_ssim = g_l1.data_ptr(), g_ssim.data_ptr()
+        elif g[0] is None:
+            return None, None, None, None, None, None, None
+        else:
+            gw = g[0].to(torch.float32)
+            if ctx.w is not None:
+                gw = gw * ctx.w      # (g (1 - lambda), -g lambda)
+            # the kernel reads the B Ll1 gradients and the B ssim gradients as two contiguous vectors
+            if B == 1:
+                p_l1 = gw.data_ptr()
+                p_ssim = p_l1 + 4 * gw.stride(-1)
+            else:
+                gw = gw.reshape(B, 2).t().contiguous()
+                p_l1, p_ssim = gw.data_ptr(), gw.data_ptr() + 4 * B
         d_images = torch.empty_like(images)
-        gptr = (C.c_void_p * B)(*[None if g is None else g.data_ptr() for g in ctx.gts])
+        gptr = (C.c_void_p * B)(*[None if t is None else t.data_ptr() for t in ctx.gts])
         _lib.call("gs_loss_backward_batched" + ctx.full, B, H, W, ctx.rows4, images.data_ptr(), gptr, temp.data_ptr(),
-                  g_l1.data_ptr(), g_ssim.data_ptr(), d_images.data_ptr(), _stream())
-        return d_images, None, None, None, None
+                  p_l1, p_ssim, d_images.data_ptr(), _stream())
+        return d_images, None, None, None, None, None, None
 
 
 def fused_l1_ssim_batched(images, gts_u8, rows4, *, deterministic=None, gt_full=False):
@@ -716,8 +656,8 @@ def fused_l1_ssim_batched(images, gts_u8, rows4, *, deterministic=None, gt_full=
     order (gs_loss_forward_batched_det), the same bits on every run.
     gt_full: gts_u8 are the views' whole (3,H,W) images, read in place at rows [row0, row1) (gs_loss_*_batched_gt_full):
     the same bits as passing the strips gt[:, row0:row1, :], without copying them out."""
-    return _FusedL1SSIMBatched.apply(images, list(gts_u8), [tuple(int(v) for v in r) for r in rows4],
-                                     deterministic_enabled(deterministic), bool(gt_full))
+    return _FusedL1SSIM.apply(images, list(gts_u8), [tuple(int(v) for v in r) for r in rows4],
+                              deterministic_enabled(deterministic), bool(gt_full), False, None)
 
 
 def get_local2j_ids_bool(image_height, image_width, rank, world_size, means2D, radii, dist_global_strategy,
@@ -756,45 +696,6 @@ def get_block_XY():
     return a.value, b.value, c.value
 
 
-class _FusedL1SSIM(torch.autograd.Function):
-    """Per-strip (Ll1, ssim) of loss_distribution.py:2536-2585 in two kernels instead of ~20."""
-
-    @staticmethod
-    def forward(ctx, image, gt_u8, row0, row1, crow0, crow1, det):
-        ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
-        image = _f32c(image, "image")
-        if gt_u8.dtype != torch.uint8 or not gt_u8.is_cuda:
-            raise TypeError("gt strip must be a CUDA uint8 tensor (3, rows, W)")
-        gt_u8 = gt_u8.contiguous()
-        _, H, W = image.shape
-        rows = row1 - row0
-        if tuple(gt_u8.shape) != (3, rows, W):
-            raise ValueError(f"gt strip must be (3,{rows},{W}), got {tuple(gt_u8.shape)}")
-        sfx = "_det" if det else ""
-        tb = _lib.query("gs_loss_temp_bytes" + sfx, rows, W)
-        temp = torch.empty((tb,), dtype=torch.uint8, device=image.device)
-        out = torch.empty((2,), dtype=torch.float32, device=image.device)
-        _lib.call("gs_loss_forward" + sfx, H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
-                  out.data_ptr(), temp.data_ptr(), tb, _stream())
-        ctx.rows = (row0, row1, crow0, crow1)
-        ctx.save_for_backward(image, gt_u8, temp)
-        return out[0], out[1]
-
-    @staticmethod
-    def backward(ctx, g_l1, g_ssim):
-        image, gt_u8, temp = ctx.saved_tensors
-        _, H, W = image.shape
-        row0, row1, crow0, crow1 = ctx.rows
-        dev = image.device
-        g_l1 = torch.zeros((), device=dev) if g_l1 is None else g_l1
-        g_ssim = torch.zeros((), device=dev) if g_ssim is None else g_ssim
-        g_l1, g_ssim = g_l1.to(torch.float32).contiguous(), g_ssim.to(torch.float32).contiguous()
-        d_image = torch.empty_like(image)
-        _lib.call("gs_loss_backward", H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
-                  temp.data_ptr(), g_l1.data_ptr(), g_ssim.data_ptr(), d_image.data_ptr(), _stream())
-        return d_image, None, None, None, None, None, None
-
-
 def fused_l1_ssim(image, gt_u8, row0, row1, count_row0=None, count_row1=None, *, deterministic=None):
     """-> (Ll1, ssim_loss) 0-dim tensors, both normalised by 3*H*W of the FULL image.
     Rows [row0,row1) of `image` (and the (3,row1-row0,W) uint8 `gt_u8`) form the window the 11x11 SSIM filter sees;
@@ -803,68 +704,8 @@ def fused_l1_ssim(image, gt_u8, row0, row1, count_row0=None, count_row1=None, *,
     deterministic: as in fused_l1_ssim_batched."""
     c0 = int(row0) if count_row0 is None else int(count_row0)
     c1 = int(row1) if count_row1 is None else int(count_row1)
-    return _FusedL1SSIM.apply(image, gt_u8, int(row0), int(row1), c0, c1, deterministic_enabled(deterministic))
-
-
-_LOSS_W = {}
-
-
-class _FusedLoss(torch.autograd.Function):
-    """(1 - lambda) Ll1 + lambda (1 - ssim) of one strip as ONE autograd node (train_internal.py:166-189 forms it with five
-    elementwise kernels and as many in the backward): the two sums come out of gs_loss_forward, the combination is one dot
-    product with a cached weight vector, and the backward hands (g (1 - lambda), -g lambda) to gs_loss_backward."""
-
-    @staticmethod
-    def forward(ctx, image, gt_u8, row0, row1, crow0, crow1, lambda_dssim, det, gt_full):
-        ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
-        image = _f32c(image, "image")
-        what = "image (3, H, W)" if gt_full else "strip (3, rows, W)"
-        if gt_u8.dtype != torch.uint8 or not gt_u8.is_cuda:
-            raise TypeError(f"gt {what} must be a CUDA uint8 tensor")
-        gt_u8 = gt_u8.contiguous()
-        _, H, W = image.shape
-        rows = row1 - row0
-        want = (3, H, W) if gt_full else (3, rows, W)
-        if tuple(gt_u8.shape) != want:
-            raise ValueError(f"gt {what} must be {want}, got {tuple(gt_u8.shape)}")
-        key = (image.device, float(lambda_dssim))
-        if key not in _LOSS_W:
-            _LOSS_W[key] = torch.tensor([1.0 - lambda_dssim, -lambda_dssim], dtype=torch.float32, device=image.device)
-        w = _LOSS_W[key]
-        sfx = "_det" if det else ""
-        out = torch.empty((2,), dtype=torch.float32, device=image.device)
-        if gt_full:   # the one-view batch of the in-place entry points: the same kernel, the same bits
-            rows4 = _i32_array([row0, row1, crow0, crow1])
-            tb = _lib.query("gs_loss_temp_bytes_batched" + sfx, 1, rows4, W)
-            temp = torch.empty((tb,), dtype=torch.uint8, device=image.device)
-            _lib.call("gs_loss_forward_batched_gt_full" + sfx, 1, H, W, rows4, image.data_ptr(),
-                      (C.c_void_p * 1)(gt_u8.data_ptr()), out.data_ptr(), temp.data_ptr(), tb, _stream())
-        else:
-            tb = _lib.query("gs_loss_temp_bytes" + sfx, rows, W)
-            temp = torch.empty((tb,), dtype=torch.uint8, device=image.device)
-            _lib.call("gs_loss_forward" + sfx, H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
-                      out.data_ptr(), temp.data_ptr(), tb, _stream())
-        ctx.rows, ctx.w, ctx.gt_full = (row0, row1, crow0, crow1), w, gt_full
-        ctx.save_for_backward(image, gt_u8, temp)
-        return torch.dot(out, w) + float(lambda_dssim)
-
-    @staticmethod
-    def backward(ctx, g):
-        image, gt_u8, temp = ctx.saved_tensors
-        _, H, W = image.shape
-        row0, row1, crow0, crow1 = ctx.rows
-        if g is None:
-            return None, None, None, None, None, None, None, None, None
-        gw = (g.to(torch.float32) * ctx.w).contiguous()      # (g (1 - lambda), -g lambda)
-        d_image = torch.empty_like(image)
-        if ctx.gt_full:
-            _lib.call("gs_loss_backward_batched_gt_full", 1, H, W, _i32_array(ctx.rows), image.data_ptr(),
-                      (C.c_void_p * 1)(gt_u8.data_ptr()), temp.data_ptr(), gw.data_ptr(), gw.data_ptr() + 4,
-                      d_image.data_ptr(), _stream())
-        else:
-            _lib.call("gs_loss_backward", H, W, row0, row1, crow0, crow1, image.data_ptr(), gt_u8.data_ptr(),
-                      temp.data_ptr(), gw.data_ptr(), gw.data_ptr() + 4, d_image.data_ptr(), _stream())
-        return d_image, None, None, None, None, None, None, None, None
+    return _FusedL1SSIM.apply(image, [gt_u8], [(int(row0), int(row1), c0, c1)], deterministic_enabled(deterministic),
+                              False, True, None)
 
 
 def fused_loss(image, gt_u8, row0, row1, lambda_dssim, count_row0=None, count_row1=None, *, deterministic=None,
@@ -874,8 +715,8 @@ def fused_loss(image, gt_u8, row0, row1, lambda_dssim, count_row0=None, count_ro
     read in place (as in fused_l1_ssim_batched)."""
     c0 = int(row0) if count_row0 is None else int(count_row0)
     c1 = int(row1) if count_row1 is None else int(count_row1)
-    return _FusedLoss.apply(image, gt_u8, int(row0), int(row1), c0, c1, float(lambda_dssim),
-                            deterministic_enabled(deterministic), bool(gt_full))
+    return _FusedL1SSIM.apply(image, [gt_u8], [(int(row0), int(row1), c0, c1)], deterministic_enabled(deterministic),
+                              bool(gt_full), True, float(lambda_dssim))
 
 
 # ---------------------------------------------------------------------------------------------------------
