@@ -122,21 +122,32 @@ def finish_strategy(history, strategies, gpu_camera_running_time, iteration, wor
     return True
 
 
+def start_strategy_whole_views(camera_uids, tile_y, world_size, global_rank):
+    """The local-sampling division (workload_division.py:858-877): with k = B / world_size views per rank, batch position
+    p is rendered whole -- tile rows [0, tile_y) -- by rank p // k.  It depends on positions only: camera_uids merely
+    label the strategies (None where a rank does not know the camera), and no cost heuristic is read or updated.
+    -> (strategies per camera, gpuid2tasks) as start_strategy."""
+    B = len(camera_uids)
+    if B % world_size:
+        raise ValueError(f"local_sampling needs bsz divisible by world size (bsz {B}, world size {world_size})")
+    per = B // world_size
+    gpuid2tasks = [[] for _ in range(world_size)]
+    strategies = []
+    for idx, uid in enumerate(camera_uids):
+        gpu = idx // per
+        gpuid2tasks[gpu].append((idx, 0, tile_y))
+        strategies.append(DivisionStrategy(uid, [gpu], [0, tile_y], tile_y, global_rank))
+    return strategies, gpuid2tasks
+
+
 def start_strategy(camera_uids, history, world_size, global_rank, border_divpos_coeff=1.0, local_sampling=False):
     """-> (strategies per camera, gpuid2tasks[gpu] = [(camera index, row_l, row_r), ...])."""
     tile_y = history.tile_y
     B = len(camera_uids)
+    if local_sampling:
+        return start_strategy_whole_views(camera_uids, tile_y, world_size, global_rank)
     gpuid2tasks = [[] for _ in range(world_size)]
     strategies = []
-    if local_sampling:
-        if B % world_size:
-            raise ValueError("local_sampling needs bsz divisible by world size")
-        per = B // world_size
-        for idx, uid in enumerate(camera_uids):
-            gpu = idx // per
-            gpuid2tasks[gpu].append((idx, 0, tile_y))
-            strategies.append(DivisionStrategy(uid, [gpu], [0, tile_y], tile_y, global_rank))
-        return strategies, gpuid2tasks
     cat = torch.cat([history.accum_heuristic[uid] for uid in camera_uids])
     pos = division_pos_heuristic(cat, world_size, right=True)
     for i in range(1, len(pos) - 1):  # snap to an image edge when closer than border_divpos_coeff rows

@@ -18,7 +18,7 @@ import torch.nn as nn
 
 from . import ops
 from .division import (DivisionStrategy, StrategyHistory, finish_strategy, heuristics_update_enabled,  # noqa: F401
-                       start_strategy)
+                       start_strategy, start_strategy_whole_views)
 
 
 class RasterSettings:
@@ -128,7 +128,8 @@ class Trainer:
     def __init__(self, scene, cams, gts_pinned, device, rank=0, world=1, lambda_dssim=0.2, group=None,
                  fused_activations=True, border_exchange=False, batched_render=True, peer_exchange=None,
                  peer_cap_rows=None, shard=None, load_balance=True, heuristic_decay=0.0,
-                 distributed_dataset_storage=False, feedback_lag=None, max_sh_degree=3, deterministic=False):
+                 distributed_dataset_storage=False, feedback_lag=None, max_sh_degree=3, deterministic=False,
+                 local_sampling=False, local_bsz=None):
         """cams, gts_pinned: the camera set -- N cameras and their uint8 (3,H,W) host images, all of one size (the reference
         keeps one global TILE_Y); each step trains on the views it lists (step(views=...)), all N by default.
         scene: the WHOLE scene (sliced here into this rank's contiguous shard), or -- shard=(lo, hi, n_total) -- only
@@ -150,8 +151,18 @@ class Trainer:
         torch.use_deterministic_algorithms.  This holds for a FIXED strip division: with more than one rank and
         load_balance=True the strips follow measured render times, which differ from run to run, so that combination is
         refused.  (The exchange sums gradients in a fixed rank order already; the NCCL all-reduce of replicated-Gaussian
-        gradient sync is outside this guarantee.)"""
-        if deterministic and world > 1 and load_balance:
+        gradient sync is outside this guarantee.)
+        local_sampling: the reference's --local_sampling (train_internal.py:113-132, workload_division.py:858-877).  Each
+        rank trains on local_bsz views of its own images per step (step(views=...)); the W * local_bsz views of all ranks
+        form the batch, and batch position p is rendered whole by rank p // local_bsz.  gts_pinned[i] is None for the
+        cameras whose images this rank does not hold; only the held images go to the device.  The ranks' view indices are
+        all-gathered on the device and the batch's camera table is gathered there from a resident (N, 40) table, so the
+        host never learns the other ranks' views.  The division reads no render times: none are gathered or fed back."""
+        self.local_sampling, self.local_bsz = bool(local_sampling), None
+        if self.local_sampling:
+            self._check_local_sampling(gts_pinned, device, world, group, local_bsz, distributed_dataset_storage,
+                                       fused_activations, batched_render, border_exchange)
+        if deterministic and world > 1 and load_balance and not self.local_sampling:
             raise ValueError("deterministic=True needs a fixed strip division: pass load_balance=False when world > 1 "
                              "(the load balancer moves the strips by measured times)")
         # None: the operators follow torch.use_deterministic_algorithms
@@ -171,6 +182,8 @@ class Trainer:
             # every splat of every local camera can land on one rank (bsz views of the scene): rows of the largest
             # receive / send total.  1.25 x the scene per view, capped by what a step can produce.
             cap = int(peer_cap_rows) if peer_cap_rows else int(1.25 * n) + 65536
+            if self.local_sampling and not peer_cap_rows:   # a rank receives its local_bsz views whole
+                cap = int(1.25 * n * self.local_bsz) + 65536
             self._peer = _ex.open_peer_buffers(world, rank, cap, device, group)
         if world > 1:
             # NCCL connects the point-to-point channels of all_to_all_single lazily, on first use: ~7 s on an 8-GPU box.  The
@@ -213,7 +226,7 @@ class Trainer:
         if gts_pinned is not None:
             if len(gts_pinned) != len(self.dcams):
                 raise ValueError(f"{len(self.dcams)} cameras but {len(gts_pinned)} ground-truth images")
-            sizes |= {(int(g.shape[-2]), int(g.shape[-1])) for g in gts_pinned}
+            sizes |= {(int(g.shape[-2]), int(g.shape[-1])) for g in gts_pinned if g is not None}
         if len(sizes) > 1:
             raise ValueError(f"all cameras and images of a Trainer must share one image size (one TILE_Y, as in the "
                              f"reference); got (H, W) = {sorted(sizes)}")
@@ -223,20 +236,66 @@ class Trainer:
         # the "inputs resident" leg keeps every image on the device (--preload_dataset_to_gpu, scene/cameras.py:67-68); its
         # loss reads the strip rows in place (ops.fused_l1_ssim_batched(gt_full=True)).  Not needed by ranks without
         # pixels in distributed-storage mode.
-        self.gts_dev = [g.to(device) for g in gts_pinned] if gts_pinned is not None else None
+        if self.local_sampling:   # only the images this rank holds
+            self.gts_dev = [None if g is None else g.to(device) for g in gts_pinned]
+        else:
+            self.gts_dev = [g.to(device) for g in gts_pinned] if gts_pinned is not None else None
         self.history = StrategyHistory([c.uid for c in self.dcams], self.tile_y, world)
         self._strip_cache = {}     # pinned copies of the strips of non-pinned host images (resident=False)
         # (N,40) host table of the batched preprocess: a step copies the rows of its views to the device
         self._cam_rows = ops.pack_cameras([c.settings() for c in self.dcams]).cpu()
         self._cams_dev = None      # (views, (B,40) device table) of the last step
+        # local sampling: the whole (N,40) table stays on the device, and a step gathers its batch's rows there
+        self._cam_table_dev = self._cam_rows.to(device) if self.local_sampling else None
+        self._whole_views = None   # ((world, rank), the whole-view division of a local-sampling batch)
         self._strategy_cache = None   # ((history version, the batch's camera uids), strategies)
         self._mask_cache = {}
         self._bmask_cache = {}
         self._n_renders = 0
         self._copy_stream = None
         self._loss_host = None
+        self._local_coef = None    # local sampling: (the loss weights of the local_bsz views, the constant term)
         self._info = {}
         self._h2d = 0
+
+    def _check_local_sampling(self, gts_pinned, device, world, group, local_bsz, distributed_dataset_storage,
+                              fused_activations, batched_render, border_exchange):
+        """The construction-time refusals of local sampling, before any other collective.  local_bsz and the number of
+        images each rank holds are all-gathered first (one small collective, none at world 1) and every rank decides from
+        the gathered values, so a rank whose value differs raises together with the others instead of leaving them
+        waiting in a collective."""
+        if distributed_dataset_storage:
+            raise ValueError("local_sampling: every rank holds the images of the views it samples; "
+                             "distributed_dataset_storage has no meaning with it")
+        if not fused_activations or not batched_render or border_exchange:
+            raise ValueError("local_sampling runs the fused-activation batched preprocess and render over whole views: "
+                             "fused_activations=False, batched_render=False and border_exchange=True do not apply")
+        try:
+            k = operator.index(local_bsz)
+        except TypeError:
+            k = 0   # refused below, on every rank
+        held = 0 if gts_pinned is None else sum(g is not None for g in gts_pinned)
+        every = [[k, held]]
+        if world > 1:
+            import torch.distributed as dist
+            allv = torch.empty((world * 2,), dtype=torch.int64, device=device)
+            dist.all_gather_into_tensor(allv, torch.tensor([k, held], dtype=torch.int64, device=device), group=group)
+            every = allv.reshape(world, 2).tolist()
+        ks = [int(e[0]) for e in every]
+        if ks[0] < 1 or any(v != ks[0] for v in ks):
+            raise ValueError(f"local_sampling needs one positive local_bsz on every rank, got {ks} (in rank order)")
+        if world * ks[0] > ops.MAX_VIEWS:
+            raise ValueError(f"local_sampling: a batch of world size x local_bsz = {world * ks[0]} views exceeds the "
+                             f"{ops.MAX_VIEWS} views of the batched kernels")
+        from .exchange import MAX_CAMERAS
+        if world > 1 and world * ks[0] > MAX_CAMERAS:
+            raise ValueError(f"local_sampling: the exchange carries at most {MAX_CAMERAS} views per step, "
+                             f"world size x local_bsz = {world * ks[0]}")
+        empty = [r for r, e in enumerate(every) if int(e[1]) == 0]
+        if empty:
+            raise ValueError(f"local_sampling: rank(s) {empty} hold no training image (gts_pinned[i] is the image of "
+                             f"camera i where the rank holds it, None elsewhere)")
+        self.local_bsz = ks[0]
 
     # -- ground truth strips (load_camera_from_cpu_to_all_gpu, loss_distribution.py:2395-2533) ------------
     def _strip_h2d(self, k, y0, y1):
@@ -272,13 +331,142 @@ class Trainer:
         """One forward + loss + backward over a batch of the camera set.  views: indices into the cameras, in batch
         order (a camera may appear more than once); None = all cameras in order.  The caller chooses them (the reference
         draws --bsz per step, train_internal.py:134).  resident=False copies the GT strips from pinned host memory inside
-        the step and reads the loss back (the end-to-end leg); returns the loss as a float then."""
-        views = self._batch_views(views)
+        the step and reads the loss back (the end-to-end leg); returns the loss as a float then.
+        With local_sampling, views are this rank's own local_bsz views (required), and the step is _step_local."""
+        views = self._local_views(views) if self.local_sampling else self._batch_views(views)
         ops.STEP_STREAM = torch.cuda.current_stream().cuda_stream   # every kernel of the step goes to this stream
         try:
-            return self._step(views, resident)
+            return self._step_local(views, resident) if self.local_sampling else self._step(views, resident)
         finally:
             ops.STEP_STREAM = None
+
+    def _local_views(self, views):
+        """This rank's views of a local-sampling step, refused before any collective or launch unless they are exactly
+        local_bsz cameras whose images this rank holds."""
+        if views is None:
+            raise ValueError(f"local_sampling: step(views=...) takes this rank's {self.local_bsz} views")
+        views = self._batch_views(views)
+        if len(views) != self.local_bsz:
+            raise ValueError(f"local_sampling: {len(views)} views passed, local_bsz is {self.local_bsz}")
+        missing = [v for v in views if self.gts_host[v] is None]
+        if missing:
+            raise ValueError(f"local_sampling: this rank does not hold the images of views {missing}")
+        return views
+
+    def _whole_view_division(self):
+        """The division of every local-sampling batch: position p whole on rank p // local_bsz.  It depends on positions
+        only, so it is built once (per rank and world size) and never reads the load balancer's history."""
+        key = (self.world, self.rank)
+        if self._whole_views is None or self._whole_views[0] != key:
+            B = self.world * self.local_bsz
+            self._whole_views = (key, start_strategy_whole_views([None] * B, self.tile_y, self.world, self.rank)[0])
+        return self._whole_views[1]
+
+    def _gathered_camera_table(self, views):
+        """(B,40) camera table of a local-sampling batch, built on the device: this rank's view indices are all-gathered in
+        rank order (all_gather_into_tensor, as train_internal.py:119-128, without its read-back to the host) and the rows
+        of the resident (N,40) table are picked at them.  The host never learns the other ranks' views."""
+        mine = torch.tensor(views, dtype=torch.int64).pin_memory().to(self.device, non_blocking=True)
+        if self.world > 1:
+            import torch.distributed as dist
+            idx = torch.empty((self.world * self.local_bsz,), dtype=torch.int64, device=self.device)
+            dist.all_gather_into_tensor(idx, mine, group=self.group)
+        else:
+            idx = mine
+        self._batch_index = idx                    # the batch's camera indices and table, kept until the next step
+        self._batch_table = torch.index_select(self._cam_table_dev, 0, idx)
+        return self._batch_table
+
+    def _step_local(self, views, resident):
+        """One local-sampling step.  Every rank projects its Gaussian shard into all B = W x local_bsz views of the batch
+        (the camera table gathered on the device), the exchange hands each rank the splats of its own views, and the rank
+        renders them whole in one batched render and scores them against its own images.  No timing feedback: the
+        division does not read it."""
+        self._trace_on = False
+        self._ex.TRACE = None
+        p = self.params
+        for t in p.raw_parameters():
+            t.grad = None
+        self._h2d = 0
+        ops.LAST_R_TOTAL = 0
+        k, B, H = self.local_bsz, self.world * self.local_bsz, self.H
+        strategies = self._whole_view_division()
+        rs = self.dcams[views[0]].settings(p.active_sh_degree)   # image size and background, shared by every view
+        gt_ready = []
+        if not resident:   # the whole own images from pinned host memory, on the copy stream, while the render runs
+            if self._copy_stream is None:
+                self._copy_stream = torch.cuda.Stream(device=self.device)
+            for v in views:
+                with torch.cuda.stream(self._copy_stream):
+                    d = self._strip_h2d(v, 0, H)
+                    ev = torch.cuda.Event()
+                    ev.record(self._copy_stream)
+                gt_ready.append((d, ev))
+        if B == 1:   # one view on one rank: the per-camera preprocess, as the default one-view step runs it
+            out = ops.preprocess_gaussians_raw(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation,
+                                               p._opacity, rs)
+            out[0].retain_grad()
+            self.means2D = [out[0]]
+            batched = tuple(t.unsqueeze(0) for t in out)
+        else:
+            batched = ops.preprocess_gaussians_batched(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation,
+                                                       p._opacity, self._gathered_camera_table(views), self.W, self.H,
+                                                       p.active_sh_degree)
+            batched[0].retain_grad()   # (B,P,2): densification reads the screen-space gradients of all B views
+            self.means2D = batched[0]
+        self._radii_local = batched[3]
+        if self.world > 1:
+            self._ex.PIGGYBACK_IN = None   # no render times ride on the exchange
+            cat, view_start, _cnt = self._ex.exchange_cat(*batched, strategies, [rs], self.world, self.rank, self.group,
+                                                          self._peer)
+            view_start = view_start[self.rank * k:(self.rank + 1) * k + 1]   # the other views have no rows here
+        else:
+            Pn = batched[0].shape[1]
+            cat = (batched[0].reshape(-1, 2), batched[1].reshape(-1, 3), batched[2].reshape(-1, 4),
+                   batched[3].reshape(-1), batched[4].reshape(-1))
+            view_start = [q * Pn for q in range(B + 1)]
+        collectors = [{} for _ in range(k)]
+        m2, rgb, co, radii, depths = cat
+        images, _stats = ops.render_gaussians_batched(m2, co, rgb, depths, radii, None, view_start, rs,
+                                                      {"stats_collector": collectors[0]}, deterministic=self.deterministic)
+        if resident:   # the whole resident images, read in place
+            gts = [self.gts_dev[v] for v in views]
+        else:
+            gts = []
+            for gt, ev in gt_ready:
+                torch.cuda.current_stream().wait_event(ev)
+                gt.record_stream(torch.cuda.current_stream())
+                gts.append(gt)
+        if self._local_coef is None:   # the weights and constant the default batched step forms for whole strips
+            coef, const = [], 0.0
+            for _ in range(k):
+                coef += [1.0 - self.lambda_dssim, -self.lambda_dssim]
+                const += self.lambda_dssim
+            self._local_coef = (torch.tensor(coef, dtype=torch.float32, device=self.device), const)
+        coef, const = self._local_coef
+        l1_ssim = ops.fused_l1_ssim_batched(images, gts, [(0, H, 0, H)] * k, deterministic=self.deterministic,
+                                            gt_full=resident)
+        loss_sum = torch.dot(l1_ssim.reshape(-1), coef) + const
+        loss_sum.backward()
+        self._n_renders = 1
+        self._finish_local_step(strategies, collectors, int(view_start[-1]) - int(view_start[0]))
+        if resident:
+            return None
+        return self._read_loss(loss_sum)
+
+    def _finish_local_step(self, strategies, collectors, n_splats):
+        """The host bookkeeping after a local-sampling step.  Nothing is queued for the load balancer."""
+        self._collectors, self._strategies = collectors, strategies
+        self._counts = dict(Vp=n_splats, P_local=self.local_bsz * self.H * self.W)
+        self.iteration += 1
+
+    def _read_loss(self, loss_sum):
+        """The step's loss as a float, through a pinned host word (the resident=False leg)."""
+        if self._loss_host is None:
+            self._loss_host = torch.zeros((1,), dtype=torch.float32).pin_memory()
+        self._loss_host.copy_(loss_sum.detach().reshape(1), non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return float(self._loss_host[0])
 
     def _batch_views(self, views):
         N = len(self.dcams)
@@ -507,11 +695,7 @@ class Trainer:
         self._mark("t time feedback")
         if resident:
             return None
-        if self._loss_host is None:
-            self._loss_host = torch.zeros((1,), dtype=torch.float32).pin_memory()
-        self._loss_host.copy_(loss_sum.detach().reshape(1), non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        return float(self._loss_host[0])
+        return self._read_loss(loss_sum)
 
     def _times_of(self, strategies, collectors, n_renders):
         """This rank's gpu_camera_running_time row for one step: the render time of each camera it rendered a strip of."""
