@@ -90,6 +90,9 @@ SIGNATURES = {
     "gs_loss_forward_batched_gt_full": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "gs_loss_forward_batched_gt_full_det": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "gs_loss_backward_batched_gt_full": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_eval_slot_count": (_i, [_i, _i]),
+    "gs_eval_sums_batched": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_eval_finalize": (_i, [_i, _i, _i, _vp, _vp, _vp]),
     "gs_profile_enable": (_i, [_i]),
     "gs_profile_read": (_i, [_i, C.POINTER(C.c_double), C.POINTER(_i64)]),
     "gs_profile_stage_name": (C.c_char_p, [_i]),

@@ -660,6 +660,55 @@ def fused_l1_ssim_batched(images, gts_u8, rows4, *, deterministic=None, gt_full=
                               deterministic_enabled(deterministic), bool(gt_full), False, None)
 
 
+def eval_sums_batched(images, gts, rows, gt_row0):
+    """The per-tile-row metric sums of training_report (train_internal.py:461-478) for the B views of `images` (B,3,H,W)
+    fp32 (gs_eval_sums_batched).  rows: B pairs (row0, row1) of local pixel rows (row0 a multiple of 16, row1 too or H;
+    row0 == row1: none); gts: B CUDA uint8 (3, R, W) ground truths holding image rows [gt_row0[v], gt_row0[v] + R), read
+    in place -- a whole resident image with gt_row0 0, or a strip with gt_row0 = row0 -- (None where a view has no rows).
+    -> (B, TILE_Y, 3, 2) fp64 slots: per tile row and channel (sum |clamp(x,0,1) - g/255|, sum of its square) over that
+    row's pixels, +0.0 outside the local rows.  A slot does not depend on the batch, the rank or the strip boundaries, so
+    summing the slots of the ranks gives the same bits as one rank.  No autograd."""
+    images = _f32c(images, "images")
+    if images.dim() != 4 or images.shape[1] != 3:
+        raise ValueError(f"images must be (B, 3, H, W), got {tuple(images.shape)}")
+    B, _, H, W = images.shape
+    if not (len(gts) == len(rows) == len(gt_row0) == B):
+        raise ValueError("one ground truth, one (row0, row1) and one gt_row0 per view")
+    keep, g_rows = [], []
+    for k, (gt, r) in enumerate(zip(gts, rows)):
+        if int(r[1]) == int(r[0]) and gt is None:
+            keep.append(None)
+            g_rows.append(0)
+            continue
+        if gt is None or gt.dtype != torch.uint8 or not gt.is_cuda or gt.device != images.device:
+            raise TypeError(f"gt {k} must be a uint8 tensor on {images.device}")
+        gt = gt.contiguous()
+        if gt.dim() != 3 or gt.shape[0] != 3 or gt.shape[2] != W:
+            raise ValueError(f"gt {k} must be (3, rows, {W}), got {tuple(gt.shape)}")
+        keep.append(gt)
+        g_rows.append(int(gt.shape[1]))
+    slots = torch.empty((B, (H + BLOCK_Y - 1) // BLOCK_Y, 3, 2), dtype=torch.float64, device=images.device)
+    _lib.call("gs_eval_sums_batched", B, H, W, images.data_ptr(),
+              (C.c_void_p * B)(*[None if g is None else g.data_ptr() for g in keep]), _i32_array(gt_row0),
+              _i32_array(g_rows), _i32_array([r[0] for r in rows]), _i32_array([r[1] for r in rows]), slots.data_ptr(),
+              _stream())
+    return slots
+
+
+def eval_finalize(slots, H, W):
+    """(B, TILE_Y, 3, 2) fp64 slots (eval_sums_batched, summed over the ranks) -> (B, 2) fp64 (L1, PSNR) per view:
+    L1 = sum of |.| / (3 H W) and PSNR = the mean over the channels of 20 log10(1 / sqrt(MSE_c)) (gs_eval_finalize)."""
+    if slots.dtype != torch.float64 or not slots.is_cuda:
+        raise TypeError("slots must be a CUDA float64 tensor")
+    B = slots.shape[0]
+    if tuple(slots.shape) != (B, (int(H) + BLOCK_Y - 1) // BLOCK_Y, 3, 2):
+        raise ValueError(f"slots must be (B, TILE_Y, 3, 2) for H = {H}, got {tuple(slots.shape)}")
+    slots = slots.contiguous()
+    out = torch.empty((B, 2), dtype=torch.float64, device=slots.device)
+    _lib.call("gs_eval_finalize", B, int(H), int(W), slots.data_ptr(), out.data_ptr(), _stream())
+    return out
+
+
 def get_local2j_ids_bool(image_height, image_width, rank, world_size, means2D, radii, dist_global_strategy,
                          cuda_args=None):
     """(P, world_size) bool: does splat i touch rank j's flattened tile range.  `rank` is unused (kept for

@@ -12,6 +12,7 @@ with the same partitioning rules:
 """
 
 import operator
+from types import SimpleNamespace
 
 import torch
 import torch.nn as nn
@@ -298,23 +299,21 @@ class Trainer:
         self.local_bsz = ks[0]
 
     # -- ground truth strips (load_camera_from_cpu_to_all_gpu, loss_distribution.py:2395-2533) ------------
-    def _strip_h2d(self, k, y0, y1):
-        """Rows [y0, y1) of the pinned (3,H,W) uint8 ground truth -> a (3, rows, W) device strip: the rows of one channel
-        are contiguous in the pinned image, so the strip is three asynchronous copies straight out of it -- no staging
-        copy, and nothing to re-pin when the load balancer moves the strip boundaries (a pinned staging strip per
-        division cost several ms of cudaHostAlloc every time the strips of a 4K view moved)."""
-        host = self.gts_host[k]
-        if not host.is_pinned():
-            key = (k, y0, y1, False)
+    def _strip_h2d(self, host, y0, y1, cache_key=None):
+        """Rows [y0, y1) of a (3,H,W) uint8 host image -> a (3, rows, W) device strip: the rows of one channel are
+        contiguous in the image, so the strip is three asynchronous copies straight out of a pinned image -- no staging
+        copy, and nothing to re-pin when the load balancer moves the strip boundaries (a pinned staging strip per division
+        cost several ms of cudaHostAlloc every time the strips of a 4K view moved).  A pageable image with a cache_key
+        goes through a pinned copy of the strip kept in the strip cache; without one, the three copies stage through
+        pageable memory."""
+        if not host.is_pinned() and cache_key is not None:
+            key = (cache_key, y0, y1, False)
             if key not in self._strip_cache:
                 self._strip_cache[key] = host[:, y0:y1, :].contiguous().pin_memory()
-            h = self._strip_cache[key]
-            self._h2d += h.numel()
-            return h.to(self.device, non_blocking=True)
+            return self._strip_cache[key].to(self.device, non_blocking=True)
         d = torch.empty((3, y1 - y0, self.W), dtype=torch.uint8, device=self.device)
         for c in range(3):
             d[c].copy_(host[c, y0:y1, :], non_blocking=True)
-        self._h2d += d.numel()
         return d
 
     def _mark(self, name):
@@ -339,6 +338,128 @@ class Trainer:
             return self._step_local(views, resident) if self.local_sampling else self._step(views, resident)
         finally:
             ops.STEP_STREAM = None
+
+    def evaluate(self, views=None, *, cams=None, gts=None, bsz=None):
+        """training_report's L1 / PSNR (train_internal.py:355-490) over a set of views, rendered forward-only.
+        cams / gts None: the Trainer's own cameras, scored against its own images (the reference's "train" config).
+        cams + gts: a held-out set of camera dicts of the Trainer's image size and their uint8 (3,H,W) images, on the
+        device (read in place) or on the host (pinned or not; a rank copies only its own strip rows).  With
+        distributed_dataset_storage the images are rank 0's, scattered by strip as the training step scatters them (the
+        other ranks' gts entries may be None).  views: indices into the chosen set, in order (None = all); choosing them
+        -- the reference's truncation to whole batches and its sample of the training views -- is the caller's.
+        bsz: views per batch, default all of them up to 64 on one rank and exchange.MAX_CAMERAS on several.
+
+        Each batch runs the forward of a training step (_forward) over a fresh strip division of the listed views (the
+        reference builds a fresh DivisionStrategyHistoryFinal per evaluation, :387) at the active SH degree, and
+        ops.eval_sums_batched scores the local strips per tile row.  The slots of all batches are summed over the ranks in
+        ONE all-reduce, exact because each tile row is local to one rank, and finalized on the device, so every view's
+        numbers are the same bits at any world size, strip division and bsz.  One host read, at the end.  The training
+        state -- division history, queued timing feedback, iteration, means2D / radii, gradients -- is left as it was.
+        -> {"l1", "psnr": the means over the views (floats), "l1_per_view", "psnr_per_view": (n,) float64 on the device}"""
+        from .exchange import MAX_CAMERAS
+        held_out = cams is not None or gts is not None
+        if held_out:
+            if cams is None or gts is None:
+                raise ValueError("evaluate: pass cams and gts together (a held-out set), or neither (the Trainer's own)")
+            if len(gts) != len(cams):
+                raise ValueError(f"evaluate: {len(cams)} cameras but {len(gts)} ground-truth images")
+            dcams = [DeviceCamera(c, self.device) for c in cams]
+            for dc in dcams:
+                dc.bg = self.dcams[0].bg   # the Trainer's background, as training renders it
+            sizes = {(c.image_height, c.image_width) for c in dcams}
+            sizes |= {(int(g.shape[-2]), int(g.shape[-1])) for g in gts if g is not None}
+            if sizes - {(self.H, self.W)}:
+                raise ValueError(f"evaluate: the held-out images must have the Trainer's size (H, W) = {(self.H, self.W)}, "
+                                 f"got {sorted(sizes)}")
+            for k, g in enumerate(gts):
+                if g is not None and (g.dtype != torch.uint8 or tuple(g.shape) != (3, self.H, self.W)):
+                    raise ValueError(f"evaluate: gts[{k}] must be uint8 (3, {self.H}, {self.W}), got {g.dtype} "
+                                     f"{tuple(g.shape)}")
+                if g is not None and g.is_cuda and g.device != torch.device(self.device):
+                    raise ValueError(f"evaluate: gts[{k}] is on {g.device}, the Trainer on {self.device}")
+            if (not self.distributed_dataset_storage or self.rank == 0) and any(g is None for g in gts):
+                raise ValueError("evaluate: a ground-truth image is None (only ranks other than 0 of a "
+                                 "distributed_dataset_storage Trainer may leave them out)")
+            host = list(gts)
+        else:
+            if self.gts_dev is None and not self.distributed_dataset_storage:
+                raise ValueError("evaluate: this Trainer holds no images of its cameras; pass a held-out set")
+            if self.local_sampling:
+                raise ValueError("evaluate: a local-sampling Trainer holds only its own rank's images, so it cannot score "
+                                 "its camera set; pass a held-out set (cams=..., gts=...) on every rank")
+            dcams, host = self.dcams, self.gts_host
+        N = len(dcams)
+        views = tuple(range(N)) if views is None else tuple(operator.index(v) for v in views)
+        if not views:
+            raise ValueError("evaluate: no views listed")
+        bad = [v for v in views if not 0 <= v < N]
+        if bad:
+            raise ValueError(f"evaluate: views {bad} are not in the set (0..{N - 1})")
+        cap = ops.MAX_VIEWS if self.world == 1 else MAX_CAMERAS
+        if bsz is None:
+            bsz = min(len(views), cap)
+        bsz = operator.index(bsz)
+        if not 1 <= bsz <= cap:
+            raise ValueError(f"evaluate: bsz must be in 1..{cap} at world size {self.world}, got {bsz}")
+        saved = (ops.LAST_R_TOTAL, getattr(self, "_trace_on", False), self._ex.TRACE, ops.STEP_STREAM)
+        self._trace_on, self._ex.TRACE = False, None
+        ops.STEP_STREAM = torch.cuda.current_stream().cuda_stream
+        try:
+            with torch.no_grad():
+                return self._evaluate(dcams, host, views, bsz, held_out)
+        finally:
+            ops.LAST_R_TOTAL, self._trace_on, self._ex.TRACE, ops.STEP_STREAM = saved
+
+    def _evaluate(self, dcams, host, views, bsz, held_out):
+        p, H = self.params, self.H
+        history = StrategyHistory(sorted({dcams[v].uid for v in views}), self.tile_y, self.world)
+        batches, slots = [], []
+        for b0 in range(0, len(views), bsz):
+            bviews = views[b0:b0 + bsz]
+            bcams = [dcams[v] for v in bviews]
+            strategies, tasks = start_strategy([c.uid for c in bcams], history, self.world, self.rank)
+            settings = [c.settings(p.active_sh_degree) for c in bcams]
+            # each local strip's ground truth and its first row: resident images in place, host images by strip rows
+            gts, gt_row0, rows = [], [], []
+            if self.distributed_dataset_storage:
+                from . import gt_scatter
+                strips, _ = gt_scatter.scatter_gt_strips([host[v] for v in bviews] if self.rank == 0 else self.W, tasks,
+                                                         H, self.device, self.rank, self.world, self.group)
+            for k, st in enumerate(strategies):
+                r = st.local_pixel_rows(H)
+                if r is None:
+                    gts.append(None); gt_row0.append(0); rows.append((0, 0))
+                    continue
+                rows.append(r)
+                if self.distributed_dataset_storage:
+                    gts.append(strips[k]); gt_row0.append(r[0])
+                elif not held_out:
+                    gts.append(self.gts_dev[bviews[k]]); gt_row0.append(0)
+                elif host[bviews[k]].is_cuda:
+                    gts.append(host[bviews[k]]); gt_row0.append(0)
+                else:
+                    gts.append(self._strip_h2d(host[bviews[k]], r[0], r[1])); gt_row0.append(r[0])
+            collectors = [{} for _ in bcams]
+            fw = self._forward(settings, strategies, collectors, lambda: ops.pack_cameras(settings), training=False)
+            if fw.images is not None:
+                s = ops.eval_sums_batched(fw.images, gts, rows, gt_row0)
+            else:   # per-camera renders; the slots of cameras without a strip here stay +0.0
+                s = torch.zeros((len(bcams), self.tile_y, 3, 2), dtype=torch.float64, device=self.device)
+                for k, image, _n in fw.per_camera:
+                    s[k] = ops.eval_sums_batched(image.unsqueeze(0), gts[k:k + 1], rows[k:k + 1], gt_row0[k:k + 1])[0]
+            slots.append(s)
+            batches.append(len(bcams))
+        slots = torch.cat(slots) if len(slots) > 1 else slots[0]
+        if self.world > 1:   # every tile row is non-zero on one rank only: the sum is exact in any order
+            import torch.distributed as dist
+            dist.all_reduce(slots, op=dist.ReduceOp.SUM, group=self.group)
+        per_view, b0 = [], 0
+        for b in batches:
+            per_view.append(ops.eval_finalize(slots[b0:b0 + b], H, self.W))
+            b0 += b
+        per_view = torch.cat(per_view) if len(per_view) > 1 else per_view[0]
+        means = (per_view.sum(0) / len(views)).tolist()   # the call's one host read
+        return {"l1": means[0], "psnr": means[1], "l1_per_view": per_view[:, 0], "psnr_per_view": per_view[:, 1]}
 
     def _local_views(self, views):
         """This rank's views of a local-sampling step, refused before any collective or launch unless they are exactly
@@ -398,7 +519,8 @@ class Trainer:
                 self._copy_stream = torch.cuda.Stream(device=self.device)
             for v in views:
                 with torch.cuda.stream(self._copy_stream):
-                    d = self._strip_h2d(v, 0, H)
+                    d = self._strip_h2d(self.gts_host[v], 0, H, cache_key=v)
+                    self._h2d += d.numel()
                     ev = torch.cuda.Event()
                     ev.record(self._copy_stream)
                 gt_ready.append((d, ev))
@@ -517,7 +639,6 @@ class Trainer:
                 self.trace = {}
             torch.cuda.synchronize()
             self._t_last = _time.perf_counter()
-        ops_ = ops
         p = self.params
         for t in p.raw_parameters():
             t.grad = None
@@ -549,25 +670,93 @@ class Trainer:
                 if rows is None:
                     continue
                 with torch.cuda.stream(self._copy_stream):
-                    d = self._strip_h2d(views[k], rows[0], rows[1])
+                    d = self._strip_h2d(self.gts_host[views[k]], rows[0], rows[1], cache_key=views[k])
+                    self._h2d += d.numel()
                     ev = torch.cuda.Event()
                     ev.record(self._copy_stream)
                 gt_ready[k] = (d, ev)
+        collectors = [{} for _ in dcams]
+        fw = self._forward(settings, strategies, collectors, lambda: self._camera_table(views), training=True)
+        self.means2D, self._radii_local, self._n_renders = fw.means2D, fw.radii, fw.n_renders
+        loss_sum = None
+        Vp = Pl = 0
+        if fw.images is not None:   # one batched render of every local strip
+            rows4, coef, const = fw.rows4, fw.coef, fw.const
+            gts = []
+            for k, (y0, y1, _c0, _c1) in enumerate(rows4):
+                if y1 == y0:
+                    gts.append(None)
+                elif resident:   # the whole resident image, read in place
+                    gts.append(self.gts_dev[views[k]])
+                else:
+                    gt, ev = gt_ready[k]
+                    torch.cuda.current_stream().wait_event(ev)
+                    gt.record_stream(torch.cuda.current_stream())
+                    gts.append(gt)
+            l1_ssim = ops.fused_l1_ssim_batched(fw.images, gts, rows4, deterministic=self.deterministic, gt_full=resident)
+            # sum over the local strips of (1 - lambda) Ll1 + lambda (1 - ssim)
+            loss_sum = torch.dot(l1_ssim.reshape(-1), coef) + const
+            Vp = int(fw.view_start[-1])
+            Pl = sum((r[1] - r[0]) * self.W for r in rows4)
+        for k, image, n_splats in fw.per_camera:
+            st = strategies[k]
+            y0, y1 = st.local_pixel_rows(self.H)
+            if self.border_exchange and self.world > 1 and len(st.gpu_ids) > 1:
+                from . import border
+                image, (r0, r1), _ = border.add_remote_border_rows(image, st, self.H, self.group)
+                loss = ops.fused_loss(image, self.gts_dev[views[k]], r0, r1, self.lambda_dssim, y0, y1,
+                                      deterministic=self.deterministic, gt_full=True)
+            else:
+                if resident:
+                    gt = self.gts_dev[views[k]]
+                else:
+                    gt, ev = gt_ready[k]
+                    torch.cuda.current_stream().wait_event(ev)
+                    gt.record_stream(torch.cuda.current_stream())
+                # a strip of every row is the resident image itself: the strip form reads it with no host-side row
+                # tables (the single-rank step); only a part of the image needs the in-place form
+                loss = ops.fused_loss(image, gt, y0, y1, self.lambda_dssim, deterministic=self.deterministic,
+                                      gt_full=resident and (y0, y1) != (0, self.H))
+            loss_sum = loss if loss_sum is None else loss_sum + loss
+            Vp += n_splats
+            Pl += (y1 - y0) * self.W
+        self._mark("r render+loss")
+        loss_sum.backward()
+        self._mark("b4 backward (rest)")
+        self._collectors, self._strategies = collectors, strategies
+        self._counts = dict(Vp=Vp, P_local=Pl)
+        self.iteration += 1
+        self._feed_back_times(strategies, collectors)
+        self._mark("t time feedback")
+        if resident:
+            return None
+        return self._read_loss(loss_sum)
+
+    def _forward(self, settings, strategies, collectors, cam_table, training):
+        """The forward of one batch, on the path the Trainer's options select: preprocess (all cameras in one batched launch
+        with fused activations, else per camera) -> exchange of the projected splats (W > 1) -> render (one batched render
+        of every local strip, else one render per camera with a strip here).  cam_table(): the (B,40) device camera table
+        of the batched preprocess.  training=False (evaluate): no screen-space gradient is retained and no render times
+        ride on the exchange.
+        -> namespace of means2D and radii (this rank's pre-exchange values, which densification reads); images (B,3,H,W)
+        of the batched render with its rows4 / coef / const / view_start, or None; per_camera [(camera index, image (3,H,W),
+        splats rendered)] of the per-camera renders; n_renders."""
+        p = self.params
         if not self.fused_activations:  # the reference's five activation kernels + cat (__init__.py:902-906)
             xyz, scaling, rotation, feats, opacity = p.get_xyz, p.get_scaling, p.get_rotation, p.get_features, p.get_opacity
-        collectors = [{} for _ in dcams]
         screen = []
         B = len(settings)
         use_batched = self.batched_render and B > 1 and not self.border_exchange
-        if self.fused_activations and len(settings) > 1:
+        if self.fused_activations and B > 1:
             # all B cameras in ONE launch: every Gaussian is read once and projected into each camera
-            bm2, brgb, bco, bradii, bdepths = ops_.preprocess_gaussians_batched(
-                p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation, p._opacity, self._camera_table(views),
+            bm2, brgb, bco, bradii, bdepths = ops.preprocess_gaussians_batched(
+                p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation, p._opacity, cam_table(),
                 self.W, self.H, p.active_sh_degree)
-            bm2.retain_grad()   # (B,P,2): densification reads bm2.grad[k] (means2D.grad of camera k, densification.py:24)
+            if training:
+                bm2.retain_grad()   # (B,P,2): densification reads bm2.grad[k] (means2D.grad of camera k, densification.py:24)
             batched = (bm2, brgb, bco, bradii, bdepths)
             if self.world == 1 and not use_batched:
-                for k in range(len(settings)):
+                for k in range(B):
                     screen.append((bm2[k], brgb[k], bco[k], bradii[k], bdepths[k]))
             settings_loop = []
         else:
@@ -575,28 +764,33 @@ class Trainer:
             settings_loop = settings
         for k, rs in enumerate(settings_loop):
             if self.fused_activations:
-                out = ops_.preprocess_gaussians_raw(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation,
-                                                    p._opacity, rs)
+                out = ops.preprocess_gaussians_raw(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation,
+                                                   p._opacity, rs)
             else:
-                out = ops_.preprocess_gaussians(xyz, scaling, rotation, feats, opacity, rs,
-                                                {"stats_collector": collectors[k]})
-            out[0].retain_grad()
+                out = ops.preprocess_gaussians(xyz, scaling, rotation, feats, opacity, rs,
+                                               {"stats_collector": collectors[k]})
+            if training:
+                out[0].retain_grad()
             screen.append(out)
-        self.means2D = batched[0] if batched is not None else [s[0] for s in screen]
+        means2D = batched[0] if batched is not None else [s[0] for s in screen]
         self._mark("p preprocess")
         if batched is None and (self.world > 1 or use_batched):
             # per-camera results (B == 1 or unfused activations): stack into (B,P,.)
             batched = tuple(torch.stack([s[q] for s in screen]) for q in range(5))
         cat = view_start = None
         if self.world > 1:
-            self._feedback_before_exchange()
+            if training:
+                self._feedback_before_exchange()
+            else:
+                self._ex.PIGGYBACK_IN = None
             if use_batched:
                 cat, view_start, cnt = self._ex.exchange_cat(*batched, strategies, settings, self.world, self.rank,
                                                              self.group, self._peer)
             else:
                 redistributed, cnt = self._ex.exchange(*batched, strategies, settings, self.world, self.rank, self.group,
                                                        self._peer)
-            self._feedback_after_exchange()
+            if training:
+                self._feedback_after_exchange()
         elif use_batched:   # (B,P,.) stacked IS the concatenation: camera k = rows [k P, (k+1) P)
             Pn = batched[0].shape[1]
             cat = (batched[0].reshape(-1, 2), batched[1].reshape(-1, 3), batched[2].reshape(-1, 4),
@@ -604,12 +798,11 @@ class Trainer:
             view_start = [k * Pn for k in range(B + 1)]
         else:
             redistributed = screen
-        self._radii_local = (batched[3] if batched is not None else
-                             screen[0][3].unsqueeze(0) if len(screen) == 1 else torch.stack([s[3] for s in screen]))
+        radii = (batched[3] if batched is not None else
+                 screen[0][3].unsqueeze(0) if len(screen) == 1 else torch.stack([s[3] for s in screen]))
         self._mark("x5 unpack")
-        loss_sum = None
-        Vp = Pl = 0
-        self._n_renders = 0
+        fw = SimpleNamespace(means2D=means2D, radii=radii, images=None, view_start=view_start, per_camera=[],
+                             n_renders=0)
         if use_batched:
             mk = tuple((tuple(st.gpu_ids), tuple(st.division_pos), st.rank) for st in strategies)
             if mk not in self._bmask_cache:
@@ -628,74 +821,27 @@ class Trainer:
                     const += self.lambda_dssim
                 self._bmask_cache[mk] = (m.reshape(B, -1), rows4,
                                          torch.tensor(coef, dtype=torch.float32, device=self.device), const)
-            cl, rows4, coef, const = self._bmask_cache[mk]
+            cl, fw.rows4, fw.coef, fw.const = self._bmask_cache[mk]
             m2, rgb, co, radii, depths = cat
-            images, _stats = ops_.render_gaussians_batched(m2, co, rgb, depths, radii, cl, view_start, settings[0],
-                                                           {"stats_collector": collectors[0]},
-                                                           deterministic=self.deterministic)
-            self._n_renders = 1
-            gts = []
-            for k, (y0, y1, _c0, _c1) in enumerate(rows4):
-                if y1 == y0:
-                    gts.append(None)
-                elif resident:   # the whole resident image, read in place
-                    gts.append(self.gts_dev[views[k]])
-                else:
-                    gt, ev = gt_ready[k]
-                    torch.cuda.current_stream().wait_event(ev)
-                    gt.record_stream(torch.cuda.current_stream())
-                    gts.append(gt)
-            l1_ssim = ops_.fused_l1_ssim_batched(images, gts, rows4, deterministic=self.deterministic, gt_full=resident)
-            # sum over the local strips of (1 - lambda) Ll1 + lambda (1 - ssim)
-            loss_sum = torch.dot(l1_ssim.reshape(-1), coef) + const
-            Vp = int(view_start[-1])
-            Pl = sum((r[1] - r[0]) * self.W for r in rows4)
-            strategies_loop = []
-        else:
-            strategies_loop = strategies
-        for k, st in enumerate(strategies_loop):
+            fw.images, _stats = ops.render_gaussians_batched(m2, co, rgb, depths, radii, cl, view_start, settings[0],
+                                                             {"stats_collector": collectors[0]},
+                                                             deterministic=self.deterministic)
+            fw.n_renders = 1
+            return fw
+        for k, st in enumerate(strategies):
             rows = st.local_rows()
             if rows is None:
                 continue
-            self._n_renders += 1
+            fw.n_renders += 1
             m2, rgb, co, radii, depths = redistributed[k]
             ck = (tuple(st.gpu_ids), tuple(st.division_pos), st.rank)
             if ck not in self._mask_cache:
                 self._mask_cache[ck] = st.get_compute_locally(self.tile_x, self.device)
             cl = self._mask_cache[ck]
-            image, *_ = ops_.render_gaussians(m2, co, rgb, depths, radii, cl, settings[k],
-                                              {"stats_collector": collectors[k]}, deterministic=self.deterministic)
-            y0, y1 = st.local_pixel_rows(self.H)
-            if self.border_exchange and self.world > 1 and len(st.gpu_ids) > 1:
-                from . import border
-                image, (r0, r1), _ = border.add_remote_border_rows(image, st, self.H, self.group)
-                loss = ops_.fused_loss(image, self.gts_dev[views[k]], r0, r1, self.lambda_dssim, y0, y1,
-                                       deterministic=self.deterministic, gt_full=True)
-            else:
-                if resident:
-                    gt = self.gts_dev[views[k]]
-                else:
-                    gt, ev = gt_ready[k]
-                    torch.cuda.current_stream().wait_event(ev)
-                    gt.record_stream(torch.cuda.current_stream())
-                # a strip of every row is the resident image itself: the strip form reads it with no host-side row
-                # tables (the single-rank step); only a part of the image needs the in-place form
-                loss = ops_.fused_loss(image, gt, y0, y1, self.lambda_dssim, deterministic=self.deterministic,
-                                       gt_full=resident and (y0, y1) != (0, self.H))
-            loss_sum = loss if loss_sum is None else loss_sum + loss
-            Vp += m2.shape[0]
-            Pl += (y1 - y0) * self.W
-        self._mark("r render+loss")
-        loss_sum.backward()
-        self._mark("b4 backward (rest)")
-        self._collectors, self._strategies = collectors, strategies
-        self._counts = dict(Vp=Vp, P_local=Pl)
-        self.iteration += 1
-        self._feed_back_times(strategies, collectors)
-        self._mark("t time feedback")
-        if resident:
-            return None
-        return self._read_loss(loss_sum)
+            image, *_ = ops.render_gaussians(m2, co, rgb, depths, radii, cl, settings[k],
+                                             {"stats_collector": collectors[k]}, deterministic=self.deterministic)
+            fw.per_camera.append((k, image, m2.shape[0]))
+        return fw
 
     def _times_of(self, strategies, collectors, n_renders):
         """This rank's gpu_camera_running_time row for one step: the render time of each camera it rendered a strip of."""

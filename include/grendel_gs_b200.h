@@ -449,6 +449,31 @@ GS_API int gs_loss_backward_batched_gt_full(int num_views, int image_height, int
                                             const float *image, const void *const *gt_u8_ptrs_host, const void *temp,
                                             const float *grad_l1, const float *grad_ssim, float *dL_dimage, void *stream);
 
+/* ---- held-out view metrics -- train_internal.py:461-478 (training_report's L1 and PSNR) ---------------------------
+ * With x^ = clamp(x, 0, 1) (NaN propagates) and g^ = g / 255 of the uint8 ground truth (the fp32 quotient, as the
+ * reference forms it), per view v and channel c: S1 = sum |x^ - g^| and S2 = sum (x^ - g^)^2 in fp64, from the exact
+ * fp64 difference of the two fp32 values; L1_v = (S1[0] + S1[1] + S1[2]) / (3 H W) and
+ * PSNR_v = mean_c 20 log10(1 / sqrt(S2[c] / (H W))) -- the per-channel PSNR averaged, +inf for an MSE of 0.
+ *
+ * gs_eval_slot_count: the number of fp64 values in the slots of num_views views, (num_views, TILE_Y, 3, 2); 0 for bad
+ * arguments.
+ * gs_eval_sums_batched: image (B,3,H,W) fp32 of a batched render, local pixel rows [row0_host[v], row1_host[v]) per view
+ * (row0 a multiple of 16, row1 a multiple of 16 or H; row0 == row1: no local rows).  gt_u8_ptrs_host[v] is a device
+ * pointer to a (3, gt_rows, W) uint8 buffer holding image rows [gt_row0, gt_row0 + gt_rows) of the view's ground truth,
+ * read in place: gt_row0 = 0, gt_rows = H for a whole resident image, gt_row0 = row0, gt_rows = row1 - row0 for a strip.
+ * It may be NULL for a view without rows.  Writes every slot: slot (v, r) = (S1, S2) per channel over tile row r's pixels,
+ * summed in an order fixed by (W, the row) alone, and +0.0 for the tile rows outside [row0, row1).  Each tile row is local
+ * to one rank only, so a SUM all-reduce of the slots over the ranks is exact in any order.
+ * gs_eval_finalize: out (B,2) fp64 = (L1_v, PSNR_v), each view's slots added in row order.
+ * All host arrays have num_views entries; bad arguments return GS_EINVAL before any launch. */
+GS_API int gs_eval_slot_count(int num_views, int image_height);
+GS_API int gs_eval_sums_batched(int num_views, int image_height, int image_width, const float *image,
+                                const void *const *gt_u8_ptrs_host, const int32_t *gt_row0_host,
+                                const int32_t *gt_rows_host, const int32_t *row0_host, const int32_t *row1_host,
+                                double *slots, void *stream);
+GS_API int gs_eval_finalize(int num_views, int image_height, int image_width, const double *slots, double *out,
+                            void *stream);
+
 /* ---- all-to-all staging -- gaussian_renderer/__init__.py:590-607,651-658 --------------------------
  * Replaces the per-(destination, camera) nonzero() + index_select + torch.cat glue around the sparse
  * all-to-all: rows of 11 floats forward (means2D 2, rgb 3, conic_opacity 4, radius as float, depth), 9 floats
