@@ -93,6 +93,9 @@ SIGNATURES = {
     "gs_eval_slot_count": (_i, [_i, _i]),
     "gs_eval_sums_batched": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gs_eval_finalize": (_i, [_i, _i, _i, _vp, _vp, _vp]),
+    "gs_quantize_u8_batched": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_image_metric_sums_batched": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_image_metric_finalize": (_i, [_i, _i, _i, _vp, _vp, _vp]),
     "gs_profile_enable": (_i, [_i]),
     "gs_profile_read": (_i, [_i, C.POINTER(C.c_double), C.POINTER(_i64)]),
     "gs_profile_stage_name": (C.c_char_p, [_i]),

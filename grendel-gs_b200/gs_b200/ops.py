@@ -709,6 +709,78 @@ def eval_finalize(slots, H, W):
     return out
 
 
+SSIM_HALO = 5   # rows of the 11 x 11 SSIM window on each side of a pixel
+
+
+def _u8_buffer(t, k, what, channels, W, device):
+    if t is None or t.dtype != torch.uint8 or not t.is_cuda or t.device != device:
+        raise TypeError(f"{what} {k} must be a uint8 tensor on {device}")
+    if not t.is_contiguous() or t.dim() != 3 or t.shape[0] != channels or t.shape[2] != W:
+        raise ValueError(f"{what} {k} must be a contiguous ({channels}, rows, {W}) tensor, got {tuple(t.shape)}")
+    return int(t.shape[1])
+
+
+def quantize_u8_batched(images, rows, outs, out_row0):
+    """render.py's clamp + save_image's 8-bit quantization of rows [row0, row1) of each of the B views of `images`
+    (B,3,H,W) fp32, written in place into outs[v] (gs_quantize_u8_batched): a contiguous CUDA uint8 (3, R, W) buffer that
+    holds image rows [out_row0[v], out_row0[v] + R) -- a window's first three channels, say (None where a view has no
+    rows).  q = uint8(clamp(fl(fl(clamp(x,0,1) * 255) + 0.5), 0, 255)), truncated, with the multiply and the add rounded
+    separately as torch's mul(255).add_(0.5) rounds them; a NaN render gives 0.  No autograd.  -> outs."""
+    images = _f32c(images, "images")
+    if images.dim() != 4 or images.shape[1] != 3:
+        raise ValueError(f"images must be (B, 3, H, W), got {tuple(images.shape)}")
+    B, _, H, W = images.shape
+    if not (len(outs) == len(rows) == len(out_row0) == B):
+        raise ValueError("one output, one (row0, row1) and one out_row0 per view")
+    o_rows = [0 if (o is None and int(r[1]) == int(r[0])) else _u8_buffer(o, k, "out", 3, W, images.device)
+              for k, (o, r) in enumerate(zip(outs, rows))]
+    _lib.call("gs_quantize_u8_batched", B, H, W, images.data_ptr(), _i32_array([r[0] for r in rows]),
+              _i32_array([r[1] for r in rows]), (C.c_void_p * B)(*[None if o is None else o.data_ptr() for o in outs]),
+              _i32_array(out_row0), _i32_array(o_rows), _stream())
+    return outs
+
+
+def image_metric_sums_batched(windows, win_row0, rows, H):
+    """The per-tile-row sums of metrics.py's SSIM and PSNR (metrics.py:26-80) for B views of height H
+    (gs_image_metric_sums_batched).  rows: B pairs (row0, row1) of local pixel rows (row0 a multiple of 16, row1 too or H;
+    row0 == row1: none); windows: B contiguous CUDA uint8 (6, R, W) windows holding image rows
+    [win_row0[v], win_row0[v] + R) of the 8-bit render (channels 0-2, quantize_u8_batched) and of the ground truth
+    (channels 3-5), covering rows [max(0, row0 - 5), min(H, row1 + 5)) (None where a view has no rows).
+    -> (B, TILE_Y, 2) fp64 slots: per tile row (sum of the fp64 SSIM map, sum of (q - g)^2) over that row's pixels, +0.0
+    outside the local rows.  A slot does not depend on the batch, the rank or the strip boundaries, so summing the slots of
+    the ranks gives the same bits as one rank.  No autograd."""
+    B = len(windows)
+    if not (len(win_row0) == len(rows) == B) or not 1 <= B <= MAX_VIEWS:
+        raise ValueError(f"1..{MAX_VIEWS} views, with one window, one win_row0 and one (row0, row1) each")
+    live = [w for w in windows if w is not None]
+    if not live:
+        raise ValueError("no view has a window")
+    dev, W = live[0].device, int(live[0].shape[-1])
+    w_rows = [0 if (w is None and int(r[1]) == int(r[0])) else _u8_buffer(w, k, "window", 6, W, dev)
+              for k, (w, r) in enumerate(zip(windows, rows))]
+    slots = torch.empty((B, (int(H) + BLOCK_Y - 1) // BLOCK_Y, 2), dtype=torch.float64, device=dev)
+    _lib.call("gs_image_metric_sums_batched", B, int(H), W,
+              (C.c_void_p * B)(*[None if w is None else w.data_ptr() for w in windows]), _i32_array(win_row0),
+              _i32_array(w_rows), _i32_array([r[0] for r in rows]), _i32_array([r[1] for r in rows]), slots.data_ptr(),
+              _stream())
+    return slots
+
+
+def image_metric_finalize(slots, H, W):
+    """(B, TILE_Y, 2) fp64 slots (image_metric_sums_batched, summed over the ranks) -> (B, 2) fp64 (SSIM, PSNR) per view:
+    SSIM = the map's sum / (3 H W) and PSNR = 20 log10(1 / sqrt(S / (255^2 3 H W))), +inf for S = 0
+    (gs_image_metric_finalize)."""
+    if slots.dtype != torch.float64 or not slots.is_cuda:
+        raise TypeError("slots must be a CUDA float64 tensor")
+    B = slots.shape[0]
+    if tuple(slots.shape) != (B, (int(H) + BLOCK_Y - 1) // BLOCK_Y, 2):
+        raise ValueError(f"slots must be (B, TILE_Y, 2) for H = {H}, got {tuple(slots.shape)}")
+    slots = slots.contiguous()
+    out = torch.empty((B, 2), dtype=torch.float64, device=slots.device)
+    _lib.call("gs_image_metric_finalize", B, int(H), int(W), slots.data_ptr(), out.data_ptr(), _stream())
+    return out
+
+
 def get_local2j_ids_bool(image_height, image_width, rank, world_size, means2D, radii, dist_global_strategy,
                          cuda_args=None):
     """(P, world_size) bool: does splat i touch rank j's flattened tile range.  `rank` is unused (kept for

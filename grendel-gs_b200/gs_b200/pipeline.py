@@ -11,6 +11,7 @@ with the same partitioning rules:
     (gaussian_renderer/__init__.py:542-698).
 """
 
+import contextlib
 import operator
 from types import SimpleNamespace
 
@@ -356,64 +357,99 @@ class Trainer:
         numbers are the same bits at any world size, strip division and bsz.  One host read, at the end.  The training
         state -- division history, queued timing feedback, iteration, means2D / radii, gradients -- is left as it was.
         -> {"l1", "psnr": the means over the views (floats), "l1_per_view", "psnr_per_view": (n,) float64 on the device}"""
+        args = self._eval_args("evaluate", views, cams, gts, bsz)
+        with self._eval_state():
+            return self._evaluate(*args)
+
+    def image_metrics(self, views=None, *, cams=None, gts=None, bsz=None, images=False):
+        """The SSIM and PSNR that render.py + metrics.py report for a trained scene (render.py:97-138,
+        metrics.py:26-80), computed on the device from forward-only strip renders.  views, cams, gts and bsz are those of
+        evaluate, and so are the refusals, the Trainer's background and active SH degree, and the untouched training state.
+
+        Each local strip is quantized to 8 bits as render.py's clamp and save_image quantize it (ops.quantize_u8_batched)
+        into a window with its ground truth; the 5 rows on each side that the 11 x 11 SSIM window reads come from the
+        neighbouring strips' owners (image_halo.exchange_halos, one all_to_all_single per batch).
+        ops.image_metric_sums_batched scores the windows per tile row in fp64, the slots of all batches are summed over
+        the ranks in ONE all-reduce, exact because each tile row is local to one rank, and finalized on the device: every
+        view's numbers are the same bits at any world size, strip division and bsz.  With images=False, one host read, at
+        the end.  images=True also gathers the 8-bit renders on rank 0 (image_halo.gather_images, batch by batch, into
+        host memory) for the caller to write; LPIPS, which needs downloaded network weights, is not computed.
+        -> {"ssim", "psnr": the means over the views (floats), "ssim_per_view", "psnr_per_view": (n,) float64 on the
+        device, "images": a list of the n uint8 (3,H,W) CPU renders in view order on rank 0 if images=True, else None}"""
+        args = self._eval_args("image_metrics", views, cams, gts, bsz)
+        with self._eval_state():
+            return self._image_metrics(*args, bool(images))
+
+    def _eval_args(self, name, views, cams, gts, bsz):
+        """The refusals of evaluate / image_metrics, from the arguments alone, before any collective or launch.
+        -> (device cameras, their images, views, bsz, held_out)."""
         from .exchange import MAX_CAMERAS
         held_out = cams is not None or gts is not None
         if held_out:
             if cams is None or gts is None:
-                raise ValueError("evaluate: pass cams and gts together (a held-out set), or neither (the Trainer's own)")
+                raise ValueError(f"{name}: pass cams and gts together (a held-out set), or neither (the Trainer's own)")
             if len(gts) != len(cams):
-                raise ValueError(f"evaluate: {len(cams)} cameras but {len(gts)} ground-truth images")
+                raise ValueError(f"{name}: {len(cams)} cameras but {len(gts)} ground-truth images")
             dcams = [DeviceCamera(c, self.device) for c in cams]
             for dc in dcams:
                 dc.bg = self.dcams[0].bg   # the Trainer's background, as training renders it
             sizes = {(c.image_height, c.image_width) for c in dcams}
             sizes |= {(int(g.shape[-2]), int(g.shape[-1])) for g in gts if g is not None}
             if sizes - {(self.H, self.W)}:
-                raise ValueError(f"evaluate: the held-out images must have the Trainer's size (H, W) = {(self.H, self.W)}, "
+                raise ValueError(f"{name}: the held-out images must have the Trainer's size (H, W) = {(self.H, self.W)}, "
                                  f"got {sorted(sizes)}")
             for k, g in enumerate(gts):
                 if g is not None and (g.dtype != torch.uint8 or tuple(g.shape) != (3, self.H, self.W)):
-                    raise ValueError(f"evaluate: gts[{k}] must be uint8 (3, {self.H}, {self.W}), got {g.dtype} "
+                    raise ValueError(f"{name}: gts[{k}] must be uint8 (3, {self.H}, {self.W}), got {g.dtype} "
                                      f"{tuple(g.shape)}")
                 if g is not None and g.is_cuda and g.device != torch.device(self.device):
-                    raise ValueError(f"evaluate: gts[{k}] is on {g.device}, the Trainer on {self.device}")
+                    raise ValueError(f"{name}: gts[{k}] is on {g.device}, the Trainer on {self.device}")
             if (not self.distributed_dataset_storage or self.rank == 0) and any(g is None for g in gts):
-                raise ValueError("evaluate: a ground-truth image is None (only ranks other than 0 of a "
+                raise ValueError(f"{name}: a ground-truth image is None (only ranks other than 0 of a "
                                  "distributed_dataset_storage Trainer may leave them out)")
             host = list(gts)
         else:
             if self.gts_dev is None and not self.distributed_dataset_storage:
-                raise ValueError("evaluate: this Trainer holds no images of its cameras; pass a held-out set")
+                raise ValueError(f"{name}: this Trainer holds no images of its cameras; pass a held-out set")
             if self.local_sampling:
-                raise ValueError("evaluate: a local-sampling Trainer holds only its own rank's images, so it cannot score "
+                raise ValueError(f"{name}: a local-sampling Trainer holds only its own rank's images, so it cannot score "
                                  "its camera set; pass a held-out set (cams=..., gts=...) on every rank")
             dcams, host = self.dcams, self.gts_host
         N = len(dcams)
         views = tuple(range(N)) if views is None else tuple(operator.index(v) for v in views)
         if not views:
-            raise ValueError("evaluate: no views listed")
+            raise ValueError(f"{name}: no views listed")
         bad = [v for v in views if not 0 <= v < N]
         if bad:
-            raise ValueError(f"evaluate: views {bad} are not in the set (0..{N - 1})")
+            raise ValueError(f"{name}: views {bad} are not in the set (0..{N - 1})")
         cap = ops.MAX_VIEWS if self.world == 1 else MAX_CAMERAS
         if bsz is None:
             bsz = min(len(views), cap)
         bsz = operator.index(bsz)
         if not 1 <= bsz <= cap:
-            raise ValueError(f"evaluate: bsz must be in 1..{cap} at world size {self.world}, got {bsz}")
+            raise ValueError(f"{name}: bsz must be in 1..{cap} at world size {self.world}, got {bsz}")
+        return dcams, host, views, bsz, held_out
+
+    @contextlib.contextmanager
+    def _eval_state(self):
+        """Forward-only scoring: no gradients, no tracing, every kernel on the current stream; the step's globals are
+        restored afterwards."""
         saved = (ops.LAST_R_TOTAL, getattr(self, "_trace_on", False), self._ex.TRACE, ops.STEP_STREAM)
         self._trace_on, self._ex.TRACE = False, None
         ops.STEP_STREAM = torch.cuda.current_stream().cuda_stream
         try:
             with torch.no_grad():
-                return self._evaluate(dcams, host, views, bsz, held_out)
+                yield
         finally:
             ops.LAST_R_TOTAL, self._trace_on, self._ex.TRACE, ops.STEP_STREAM = saved
 
-    def _evaluate(self, dcams, host, views, bsz, held_out):
+    def _eval_batches(self, dcams, host, views, bsz, held_out):
+        """The batches of an evaluation, bsz views each: a fresh strip division of the listed views (one history per
+        call), each local strip's ground truth, and the forward.  Yields (strategies, rows, gts, gt_row0, fw) per batch:
+        rows[k] the local pixel rows of view k ((0, 0): none); gts[k] a device image holding rows [gt_row0[k], ...) of its
+        ground truth -- a resident image in place, or a strip -- or None; fw the _forward namespace."""
         p, H = self.params, self.H
         history = StrategyHistory(sorted({dcams[v].uid for v in views}), self.tile_y, self.world)
-        batches, slots = [], []
         for b0 in range(0, len(views), bsz):
             bviews = views[b0:b0 + bsz]
             bcams = [dcams[v] for v in bviews]
@@ -441,25 +477,76 @@ class Trainer:
                     gts.append(self._strip_h2d(host[bviews[k]], r[0], r[1])); gt_row0.append(r[0])
             collectors = [{} for _ in bcams]
             fw = self._forward(settings, strategies, collectors, lambda: ops.pack_cameras(settings), training=False)
-            if fw.images is not None:
-                s = ops.eval_sums_batched(fw.images, gts, rows, gt_row0)
-            else:   # per-camera renders; the slots of cameras without a strip here stay +0.0
-                s = torch.zeros((len(bcams), self.tile_y, 3, 2), dtype=torch.float64, device=self.device)
-                for k, image, _n in fw.per_camera:
-                    s[k] = ops.eval_sums_batched(image.unsqueeze(0), gts[k:k + 1], rows[k:k + 1], gt_row0[k:k + 1])[0]
-            slots.append(s)
-            batches.append(len(bcams))
-        slots = torch.cat(slots) if len(slots) > 1 else slots[0]
+            yield strategies, rows, gts, gt_row0, fw
+
+    def _sum_slots_over_ranks(self, slots):
         if self.world > 1:   # every tile row is non-zero on one rank only: the sum is exact in any order
             import torch.distributed as dist
             dist.all_reduce(slots, op=dist.ReduceOp.SUM, group=self.group)
+        return slots
+
+    def _evaluate(self, dcams, host, views, bsz, held_out):
+        batches, slots = [], []
+        for strategies, rows, gts, gt_row0, fw in self._eval_batches(dcams, host, views, bsz, held_out):
+            if fw.images is not None:
+                s = ops.eval_sums_batched(fw.images, gts, rows, gt_row0)
+            else:   # per-camera renders; the slots of cameras without a strip here stay +0.0
+                s = torch.zeros((len(strategies), self.tile_y, 3, 2), dtype=torch.float64, device=self.device)
+                for k, image, _n in fw.per_camera:
+                    s[k] = ops.eval_sums_batched(image.unsqueeze(0), gts[k:k + 1], rows[k:k + 1], gt_row0[k:k + 1])[0]
+            slots.append(s)
+            batches.append(len(strategies))
+        slots = self._sum_slots_over_ranks(torch.cat(slots) if len(slots) > 1 else slots[0])
         per_view, b0 = [], 0
         for b in batches:
-            per_view.append(ops.eval_finalize(slots[b0:b0 + b], H, self.W))
+            per_view.append(ops.eval_finalize(slots[b0:b0 + b], self.H, self.W))
             b0 += b
         per_view = torch.cat(per_view) if len(per_view) > 1 else per_view[0]
         means = (per_view.sum(0) / len(views)).tolist()   # the call's one host read
         return {"l1": means[0], "psnr": means[1], "l1_per_view": per_view[:, 0], "psnr_per_view": per_view[:, 1]}
+
+    def _image_metrics(self, dcams, host, views, bsz, held_out, images):
+        from . import image_halo
+        H, W = self.H, self.W
+        batches, slots, pictures = [], [], []
+        for strategies, rows, gts, gt_row0, fw in self._eval_batches(dcams, host, views, bsz, held_out):
+            # per local strip a (6, rows, W) window of the strip and its halo: 8-bit render in channels 0-2, ground truth
+            # in 3-5; the strip's own rows filled here, the halo rows by the neighbours' owners
+            wins, win_row0 = [], []
+            for k, (y0, y1) in enumerate(rows):
+                if y1 == y0:
+                    wins.append(None); win_row0.append(0)
+                    continue
+                a, b = image_halo.window_rows((y0, y1), H)
+                win = torch.empty((6, b - a, W), dtype=torch.uint8, device=self.device)
+                win[3:, y0 - a:y1 - a].copy_(gts[k][:, y0 - gt_row0[k]:y1 - gt_row0[k]])
+                wins.append(win); win_row0.append(a)
+            if fw.images is not None:
+                ops.quantize_u8_batched(fw.images, rows, [None if w is None else w[:3] for w in wins], win_row0)
+            for k, image, _n in fw.per_camera:
+                ops.quantize_u8_batched(image.unsqueeze(0), rows[k:k + 1], [wins[k][:3]], win_row0[k:k + 1])
+            if self.world > 1:
+                image_halo.exchange_halos(wins, win_row0, strategies, H, W, self.rank, self.world, self.group, self.device)
+            if any(w is not None for w in wins):
+                slots.append(ops.image_metric_sums_batched(wins, win_row0, rows, H))
+            else:   # no strip of this batch here: every slot is +0.0
+                slots.append(torch.zeros((len(rows), self.tile_y, 2), dtype=torch.float64, device=self.device))
+            batches.append(len(strategies))
+            if images:
+                strips = [None if w is None else w[:3, y0 - a:y1 - a]
+                          for w, a, (y0, y1) in zip(wins, win_row0, rows)]
+                got = image_halo.gather_images(strips, strategies, H, W, self.rank, self.world, self.group, self.device)
+                if got is not None:
+                    pictures.extend(got)
+        slots = self._sum_slots_over_ranks(torch.cat(slots) if len(slots) > 1 else slots[0])
+        per_view, b0 = [], 0
+        for b in batches:
+            per_view.append(ops.image_metric_finalize(slots[b0:b0 + b], H, W))
+            b0 += b
+        per_view = torch.cat(per_view) if len(per_view) > 1 else per_view[0]
+        means = (per_view.sum(0) / len(views)).tolist()   # the call's one host read; the image copies are complete too
+        return {"ssim": means[0], "psnr": means[1], "ssim_per_view": per_view[:, 0], "psnr_per_view": per_view[:, 1],
+                "images": pictures if images and (self.rank == 0 or self.world == 1) else None}
 
     def _local_views(self, views):
         """This rank's views of a local-sampling step, refused before any collective or launch unless they are exactly

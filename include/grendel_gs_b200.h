@@ -474,6 +474,35 @@ GS_API int gs_eval_sums_batched(int num_views, int image_height, int image_width
 GS_API int gs_eval_finalize(int num_views, int image_height, int image_width, const double *slots, double *out,
                             void *stream);
 
+/* ---- image metrics -- render.py:127-138 + metrics.py:26-80 (the 8-bit renders' SSIM and PSNR) ---------------------
+ * q = uint8(clamp(fl(fl(clamp(x, 0, 1) * 255) + 0.5), 0, 255)), truncated: render.py's clamp and save_image's
+ * quantization, two separately rounded fp32 operations; a NaN render gives 0.  With a = fl32(q / 255) and
+ * b = fl32(g / 255) of the uint8 ground truth g (tf.to_tensor), in fp64: the SSIM map of utils/loss_utils.py:56-80 with
+ * the separable window gaussian(11, 1.5) (the fp32 taps torch builds, promoted), zero outside the image, C1 = 0.01^2 and
+ * C2 = 0.03^2; SSIM_v = the map's sum / (3 H W); S = sum (q - g)^2 and PSNR_v = 20 log10(1 / sqrt(S / (255^2 3 H W))),
+ * the MSE pooled over the channels (+inf for S = 0).
+ *
+ * gs_quantize_u8_batched: image (B,3,H,W) fp32; per view, rows [row0_host[v], row1_host[v]) (row0 == row1: none) are
+ * quantized into the device buffer out_u8_ptrs_host[v], (3, out_rows, W) uint8 holding image rows
+ * [out_row0, out_row0 + out_rows) (NULL allowed for a view without rows).
+ * gs_image_metric_sums_batched: per view, local pixel rows [row0, row1) (row0 a multiple of 16, row1 a multiple of 16 or
+ * H; row0 == row1: none) and a device window win_u8_ptrs_host[v], (6, win_rows, W) uint8 holding image rows
+ * [win_row0, win_row0 + win_rows) of q (channels 0-2) and g (channels 3-5).  The window must cover the halo of the local
+ * rows, [max(0, row0 - 5), min(H, row1 + 5)).  Writes every slot, (B, TILE_Y, 2) fp64: slot (v, r) = (sum of the SSIM
+ * map, S) over tile row r's pixels, summed in an order fixed by (W, the row) alone, and +0.0 for the tile rows outside
+ * [row0, row1).  Each tile row is local to one rank only, so a SUM all-reduce of the slots over the ranks is exact.
+ * gs_image_metric_finalize: out (B,2) fp64 = (SSIM_v, PSNR_v), each view's slots added in row order.
+ * All host arrays have num_views entries; bad arguments return GS_EINVAL before any launch. */
+GS_API int gs_quantize_u8_batched(int num_views, int image_height, int image_width, const float *image,
+                                  const int32_t *row0_host, const int32_t *row1_host, void *const *out_u8_ptrs_host,
+                                  const int32_t *out_row0_host, const int32_t *out_rows_host, void *stream);
+GS_API int gs_image_metric_sums_batched(int num_views, int image_height, int image_width,
+                                        const void *const *win_u8_ptrs_host, const int32_t *win_row0_host,
+                                        const int32_t *win_rows_host, const int32_t *row0_host, const int32_t *row1_host,
+                                        double *slots, void *stream);
+GS_API int gs_image_metric_finalize(int num_views, int image_height, int image_width, const double *slots, double *out,
+                                    void *stream);
+
 /* ---- all-to-all staging -- gaussian_renderer/__init__.py:590-607,651-658 --------------------------
  * Replaces the per-(destination, camera) nonzero() + index_select + torch.cat glue around the sparse
  * all-to-all: rows of 11 floats forward (means2D 2, rgb 3, conic_opacity 4, radius as float, depth), 9 floats
