@@ -81,6 +81,34 @@ class GaussianParams(nn.Module):
         self.max_sh_degree = int(max_sh_degree)
         self.active_sh_degree = self.max_sh_degree
 
+    RAW_SHAPES = {"xyz": (3,), "f_dc": (1, 3), "opacity": (1,), "scaling": (3,), "rotation": (4,)}
+
+    @classmethod
+    def from_raw(cls, raw, device):
+        """The six raw parameters as they are stored (a PLY shard or a checkpoint, model_io): raw = {group name (Trainer.
+        GROUP_OF): tensor}, taken bit for bit, with no activation inverted.  max_sh_degree comes from _features_rest's
+        (P, (D+1)^2 - 1, 3); active_sh_degree starts at it."""
+        if set(raw) != set(Trainer.GROUP_OF):
+            raise ValueError(f"raw parameters need the groups {sorted(Trainer.GROUP_OF)}, got {sorted(raw)}")
+        P = int(raw["xyz"].shape[0])
+        for name, tail in cls.RAW_SHAPES.items():
+            if tuple(raw[name].shape) != (P,) + tail:
+                raise ValueError(f"raw parameter {name} must be {(P,) + tail}, got {tuple(raw[name].shape)}")
+        Km1 = raw["f_rest"].shape[1] if raw["f_rest"].dim() == 3 else -1
+        if raw["f_rest"].dim() != 3 or tuple(raw["f_rest"].shape) != (P, Km1, 3) or Km1 + 1 not in (1, 4, 9, 16):
+            raise ValueError(f"raw parameter f_rest must be (P, (D+1)^2 - 1, 3) for D = 0..3, got "
+                             f"{tuple(raw['f_rest'].shape)}")
+        self = cls.__new__(cls)
+        nn.Module.__init__(self)
+        for name, attr in Trainer.GROUP_OF.items():
+            t = raw[name].detach().to(device=device, dtype=torch.float32)
+            if not t.is_contiguous() or t.storage_offset() != 0:   # the kernels need 16-byte aligned, dense rows
+                t = t.clone(memory_format=torch.contiguous_format)
+            setattr(self, attr, nn.Parameter(t))
+        self.max_sh_degree = int(round((Km1 + 1) ** 0.5)) - 1
+        self.active_sh_degree = self.max_sh_degree
+        return self
+
     @property
     def get_xyz(self):
         return self._xyz
@@ -131,7 +159,7 @@ class Trainer:
                  fused_activations=True, border_exchange=False, batched_render=True, peer_exchange=None,
                  peer_cap_rows=None, shard=None, load_balance=True, heuristic_decay=0.0,
                  distributed_dataset_storage=False, feedback_lag=None, max_sh_degree=3, deterministic=False,
-                 local_sampling=False, local_bsz=None):
+                 local_sampling=False, local_bsz=None, model=None):
         """cams, gts_pinned: the camera set -- N cameras and their uint8 (3,H,W) host images, all of one size (the reference
         keeps one global TILE_Y); each step trains on the views it lists (step(views=...)), all N by default.
         scene: the WHOLE scene (sliced here into this rank's contiguous shard), or -- shard=(lo, hi, n_total) -- only
@@ -159,7 +187,12 @@ class Trainer:
         form the batch, and batch position p is rendered whole by rank p // local_bsz.  gts_pinned[i] is None for the
         cameras whose images this rank does not hold; only the held images go to the device.  The ranks' view indices are
         all-gathered on the device and the batch's camera table is gathered there from a resident (N, 40) table, so the
-        host never learns the other ranks' views.  The division reads no render times: none are gathered or fed back."""
+        host never learns the other ranks' views.  The division reads no render times: none are gathered or fed back.
+        model: instead of an activated scene (scene=None), this rank's six raw parameters as stored -- {group name
+        (GROUP_OF): tensor}, a shard of a PLY or checkpoint from model_io -- taken bit for bit (GaussianParams.from_raw);
+        max_sh_degree then comes from their shape and the argument is not read.  shard=(lo, hi, n_total) gives the whole
+        model's size; without it n_total is this rank's count at world size 1, and their sum over the ranks (one small
+        all-reduce) otherwise."""
         self.local_sampling, self.local_bsz = bool(local_sampling), None
         if self.local_sampling:
             self._check_local_sampling(gts_pinned, device, world, group, local_bsz, distributed_dataset_storage,
@@ -179,7 +212,12 @@ class Trainer:
             import os as _os
             peer_exchange = _os.environ.get("GS_B200_EXCHANGE", "p2p") != "nccl"
         self._peer = None
-        n = scene["means3D"].shape[0] if shard is None else int(shard[2])
+        if model is not None:
+            if scene is not None:
+                raise ValueError("pass an activated scene or the raw parameters (model=...), not both")
+            n = self._model_total(model, shard, device, world, group)
+        else:
+            n = scene["means3D"].shape[0] if shard is None else int(shard[2])
         if world > 1 and peer_exchange:
             # every splat of every local camera can land on one rank (bsz views of the scene): rows of the largest
             # receive / send total.  1.25 x the scene per view, capped by what a step can produce.
@@ -202,7 +240,10 @@ class Trainer:
         self.lambda_dssim = lambda_dssim
         self.fused_activations = fused_activations
         self.border_exchange = border_exchange   # legacy row L1: exchange 5 halo rows so strip losses sum to the full-image loss
-        if shard is None:
+        if model is not None:
+            self.params = GaussianParams.from_raw(model, device)
+            lo, hi = 0, self.params._xyz.shape[0]
+        elif shard is None:
             lo, hi = n * rank // world, n * (rank + 1) // world
             self.params = GaussianParams({k: v[lo:hi] for k, v in scene.items()}, device, max_sh_degree)
         else:
@@ -259,6 +300,22 @@ class Trainer:
         self._local_coef = None    # local sampling: (the loss weights of the local_bsz views, the constant term)
         self._info = {}
         self._h2d = 0
+
+    @staticmethod
+    def _model_total(model, shard, device, world, group):
+        """n_total of a Trainer built from raw parameters (the peer buffers are sized from it)."""
+        P = int(model["xyz"].shape[0])
+        if shard is not None:
+            if int(shard[1]) - int(shard[0]) != P:
+                raise ValueError(f"shard=(lo, hi, n_total) = {tuple(shard)} does not match the {P} Gaussians passed")
+            return int(shard[2])
+        if world == 1:
+            return P
+        import torch.distributed as dist
+        dev = device if dist.get_backend(group) == "nccl" else "cpu"
+        t = torch.tensor([P], dtype=torch.int64, device=dev)
+        dist.all_reduce(t, group=group)
+        return int(t.item())
 
     def _check_local_sampling(self, gts_pinned, device, world, group, local_bsz, distributed_dataset_storage,
                               fused_activations, batched_render, border_exchange):

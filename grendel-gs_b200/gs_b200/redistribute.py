@@ -20,6 +20,18 @@ from .exchange import all_to_all_single
 NAMES = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation")
 
 
+def fused_rows(tensors, order=None):
+    """(P, ...) tensors -> (one (P, sum of widths) tensor whose row i is row i of every tensor, flattened and side by side,
+    widths).  order: optional (P,) row indices, applied to the fused rows.  The one packing of a Gaussian's state into a
+    row, for the redistribution's all-to-all and for model_io's PLY rows."""
+    P = tensors[0].shape[0]
+    widths = [int(np.prod(t.shape[1:])) if t.dim() > 1 else 1 for t in tensors]
+    rows = torch.cat([t.reshape(P, w) for t, w in zip(tensors, widths)], dim=1)
+    if order is not None:
+        rows = rows.index_select(0, order)
+    return rows.contiguous(), widths
+
+
 def need_redistribute(n_local, group=None, threshold=7.0, first_after_densify=False):
     """gaussian_model.py:1247-1259: after the first densification, or when min * threshold < max over the ranks."""
     W = dist.get_world_size(group)
@@ -65,9 +77,8 @@ def redistribute(optimizer, destination=None, group=None, generator=None):
             tensors.append(params[k].detach())
             if has_state[k]:
                 tensors += [st["exp_avg"], st["exp_avg_sq"]]
-        widths = [int(np.prod(t.shape[1:])) if t.dim() > 1 else 1 for t in tensors]
         order = torch.sort(destination, stable=True).indices
-        send = torch.cat([t.reshape(P, w) for t, w in zip(tensors, widths)], dim=1).index_select(0, order).contiguous()
+        send, widths = fused_rows(tensors, order)
         n_new = int(sum(recv_splits))
         recv = torch.empty((n_new, send.shape[1]), dtype=send.dtype, device=dev)
         all_to_all_single(recv, send, recv_splits, send_splits, group)
