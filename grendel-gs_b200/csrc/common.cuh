@@ -48,6 +48,13 @@ GS_D void gs_get_rect(float px, float py, int r, int gx, int gy, int &x0, int &y
     y1 = min(gy, max(0, (int)(__fdiv_rn(__fadd_rn(__fadd_rn(py, rr), (float)(GS_BLOCK_Y - 1)), (float)GS_BLOCK_Y))));
 }
 
+// ---- the reference's ground-truth unit ---------------------------------------------------------------------------
+// The reference forms its ground truth as original_image / 255.0 on a CUDA uint8 tensor (gaussian_renderer/
+// loss_distribution.py:232, 938, 1469, 1833, 1933, 2107, 2224, 2269, 2561; train_internal.py:472-474; render.py:128).
+// On the device torch's true division by a scalar multiplies by the scalar's fp32 reciprocal, so that value is
+// fl32(g * fl32(1/255)), not the IEEE quotient fl32(g / 255): the two differ by one ulp on 126 of the 256 bytes.
+GS_D float gs_gt_unit(uint8_t g) { return __fmul_rn((float)g, 1.0f / 255.0f); }
+
 // ---- several views (cameras) binned and blended by ONE launch per stage --------------------------------
 // The splats of view v are rows [start[v], start[v+1]) of the concatenated splat arrays; its tiles are
 // [v*T, (v+1)*T) of the concatenated tile arrays (compute_locally, ranges) and of the sort key.  A rank that owns a

@@ -4,7 +4,8 @@
 //   Ll1  = sum |x - y|      / (3 H W)          (pixelwise_l1_with_mask, mask == all ones in the live path)
 //   ssim = sum ssim_map(x,y) / (3 H W)          (11x11 Gaussian window sigma 1.5, ZERO padding at the strip
 //                                               edges -- the live path exchanges no halo)
-// with x = rendered strip rows [row0,row1) of the full (3,H,W) image, y = clamp(gt_u8/255, 0, 1).
+// with x = rendered strip rows [row0,row1) of the full (3,H,W) image, y = clamp(gt_u8/255, 0, 1), the quotient as the
+// reference forms it on the device (gs_gt_unit: fl32(gt * fl32(1/255))).
 // The window is applied separably (row pass then column pass) from shared memory, four outputs per thread from a
 // 14-value sliding window in registers.
 //
@@ -81,7 +82,7 @@ k_loss_fwd(int W, int H, const LossViews lv, const float *__restrict__ image, fl
             float vx = 0.f, vy = 0.f;
             if (y >= 0 && y < rows && x >= 0 && x < W) {
                 vx = image[ch * HW + (size_t)(row0 + y) * W + x];
-                vy = fminf(1.f, fmaxf(0.f, (float)gt[ch * GS + (size_t)y * W + x] / 255.0f));
+                vy = fminf(1.f, fmaxf(0.f, gs_gt_unit(gt[ch * GS + (size_t)y * W + x])));
             }
             s_x[r][c] = vx; s_y[r][c] = vy;
         }
@@ -244,7 +245,7 @@ k_loss_bwd(int W, int H, const LossViews lv, const float *__restrict__ image, co
                 if (y < rows && x < W) {
                     const size_t oi = ch * HW + (size_t)(row0 + y) * W + x;
                     const float vx = image[oi];
-                    const float vy = fminf(1.f, fmaxf(0.f, (float)gt[ch * GS + (size_t)y * W + x] / 255.0f));
+                    const float vy = fminf(1.f, fmaxf(0.f, gs_gt_unit(gt[ch * GS + (size_t)y * W + x])));
                     const float d = vx - vy;
                     const float sgn = (y < crow0 || y >= crow1) ? 0.f : (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f));
                     dimg[oi] = gl1 * sgn + gss * (b0[q] + 2.f * vx * b1[q] + vy * b2[q]);

@@ -1,6 +1,6 @@
 // Held-out view metrics: the L1 and PSNR that training_report prints (train_internal.py:461-481), from per-tile-row sums.
 //   x^ = clamp(x, 0, 1)  (train_internal.py:471; NaN stays NaN, as torch.clamp leaves it)
-//   g^ = g / 255          (:472-474, the uint8 ground truth; the fp32 quotient the reference forms)
+//   g^ = g / 255          (:472-474, the uint8 ground truth divided on the device: fl32(g * fl32(1/255)), gs_gt_unit)
 //   S1[v,c] = sum |x^ - g^|,  S2[v,c] = sum (x^ - g^)^2          (fp64; x^ - g^ of two fp32 values is exact in fp64,
 //                                                                 so a render equal to the ground truth scores 0)
 //   L1_v   = (S1[v,0] + S1[v,1] + S1[v,2]) / (3 H W)             (l1_loss(...).mean(), utils/loss_utils.py:18-19)
@@ -38,7 +38,7 @@ k_eval_sums(int H, int W, const EvalViews ev, const float *__restrict__ image, d
         if (threadIdx.x < 6) out[threadIdx.x] = 0.0;
         return;
     }
-    for (int i = threadIdx.x; i < 256; i += EV_THREADS) s_g[i] = (double)__fdiv_rn((float)i, 255.f);
+    for (int i = threadIdx.x; i < 256; i += EV_THREADS) s_g[i] = (double)gs_gt_unit((uint8_t)i);
     __syncthreads();
     const size_t HW = (size_t)H * W, GP = (size_t)ev.gt_rows[view] * W;
     const int n = (y1 - y0) * W;
@@ -232,6 +232,7 @@ k_image_metric_sums(int H, int W, const MetricViews mv, double *__restrict__ slo
         if (threadIdx.x < 2) out[threadIdx.x] = 0.0;
         return;
     }
+    // the IEEE quotient, not gs_gt_unit: metrics.py's tf.to_tensor divides on the CPU
     for (int i = threadIdx.x; i < 256; i += IM_THREADS) s_val[i] = (double)__fdiv_rn((float)i, 255.f);
     const uint8_t *__restrict__ win = mv.win[view];
     const size_t WP = (size_t)mv.win_rows[view] * W;
@@ -276,10 +277,14 @@ k_image_metric_sums(int H, int W, const MetricViews mv, double *__restrict__ slo
                     e22 = fma(w, s_h[3][tr + k][tc], e22);
                     e12 = fma(w, s_h[4][tr + k][tc], e12);
                 }
-                const double mu1_sq = mu1 * mu1, mu2_sq = mu2 * mu2, mu1_mu2 = mu1 * mu2;
-                const double s11 = e11 - mu1_sq, s22 = e22 - mu2_sq, s12 = e12 - mu1_mu2;
+                // each operation rounded on its own, as _ssim writes them: no FMA contraction, so a == b gives
+                // numerator == denominator and a map of exactly 1 (a render whose 8-bit image is the ground truth)
+                const double mu1_sq = __dmul_rn(mu1, mu1), mu2_sq = __dmul_rn(mu2, mu2), mu1_mu2 = __dmul_rn(mu1, mu2);
+                const double s11 = __dsub_rn(e11, mu1_sq), s22 = __dsub_rn(e22, mu2_sq), s12 = __dsub_rn(e12, mu1_mu2);
                 const double C1 = 0.01 * 0.01, C2 = 0.03 * 0.03;
-                acc_map += ((2.0 * mu1_mu2 + C1) * (2.0 * s12 + C2)) / ((mu1_sq + mu2_sq + C1) * (s11 + s22 + C2));
+                const double num = __dmul_rn(__dadd_rn(2.0 * mu1_mu2, C1), __dadd_rn(2.0 * s12, C2));
+                const double den = __dmul_rn(__dadd_rn(__dadd_rn(mu1_sq, mu2_sq), C1), __dadd_rn(__dadd_rn(s11, s22), C2));
+                acc_map += num / den;
                 const size_t at = (size_t)(y - wr0) * W + x;
                 const int d = (int)win[c * WP + at] - (int)win[(3 + c) * WP + at];
                 acc_sse += (double)(d * d);

@@ -1,10 +1,11 @@
 """Images and ground truth for the strip loss kernels (csrc/loss.cu), by regime, and the windows they are cut into.
 
 Regimes, each measured by `regimes()` on the data itself rather than trusted to the generator:
-  equal          x == fl32(gt / 255): |x - y| has no sign, its gradient must be 0 (torch's abs)
+  equal          x == y = fl32(gt * fl32(1/255)), the reference's gt / 255.0 on the device: |x - y| has no sign, its
+                 gradient must be 0 (torch's abs)
   equal_zero     x == y == 0: a black background rendered over black ground truth
   equal_one      x == y == 1 on gt 255
-  ulp_above / ulp_below   x one fp32 ulp either side of fl32(gt / 255)
+  ulp_above / ulp_below   x one fp32 ulp either side of y
   flat_both / flat_x / flat_y   an 11x11 neighbourhood inside the image where both / only x / only y are constant: the
                  SSIM variances vanish (both: sigma1 = sigma2 = 0)
   saturated      x > 1 (rendered rgb is not clamped above), up to ~2.5
@@ -15,13 +16,16 @@ Regimes, each measured by `regimes()` on the data itself rather than trusted to 
 import numpy as np
 from scipy import ndimage
 
+from eval_ref import INV255
+
 REGIMES = ("equal", "equal_zero", "equal_one", "ulp_above", "ulp_below", "flat_both", "flat_x", "flat_y", "saturated",
            "negative", "checker", "smooth")
 
 
 def gt_float(gt):
-    """The ground truth as the kernel sees it: clamp(fl32(gt / 255), 0, 1)."""
-    return np.clip(gt.astype(np.float32) / np.float32(255), 0, 1)
+    """The ground truth as the kernel sees it: clamp(fl32(gt * fl32(1/255)), 0, 1), the reference's gt / 255.0 on the
+    device (eval_ref.gt_hat)."""
+    return np.clip(gt.astype(np.float32) * INV255, 0, 1)
 
 
 def _smooth(rng, H, W):

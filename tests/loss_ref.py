@@ -57,7 +57,8 @@ def counted_terms(img, y_win, row0, row1, c0, c1, dtype=torch.float64):
 def strip_loss(img, y_win, row0, row1, c0, c1, g_l1, g_ssim, dtype=torch.float64):
     """The kernel's contract on one view, evaluated in `dtype` on img's device, one channel at a time (the channels are
     independent; this keeps a 3840x2160 fp64 graph near 1 GiB).
-    img: (3, H, W) tensor or array; y_win: (3, row1 - row0, W) ground truth as the kernel sees it (fl32(gt / 255));
+    img: (3, H, W) tensor or array; y_win: (3, row1 - row0, W) ground truth as the kernel sees it: the reference's
+    gt / 255.0 on the device, fl32(gt * fl32(1/255)) (loss_cases.gt_float);
     rows absolute.  -> (Ll1, ssim, d(g_l1 Ll1 + g_ssim ssim) / d img as a (3, H, W) tensor)."""
     img = torch.as_tensor(img)
     y_win = torch.as_tensor(y_win).to(img.device)

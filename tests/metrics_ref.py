@@ -71,6 +71,36 @@ def slots(q, g, rows=None):
     return out
 
 
+def slots_torch(q, g, rows=None):
+    """slots() in torch float64 on the tensors' device, for images too large for numpy: (3,H,W) uint8 tensors q and g
+    on one device -> (TILE_Y, 2) float64 tensor.  a and b come from a table of unit() built on the CPU: on a GPU torch's
+    u8 / 255 would multiply by fl32(1/255) instead of dividing."""
+    H, W = q.shape[1:]
+    row0, row1 = (0, H) if rows is None else rows
+    table = torch.from_numpy(unit(np.arange(256, dtype=np.uint8))).to(q.device)
+    a, b = table[q.long()], table[g.long()]
+    w = torch.tensor(WINDOW, dtype=torch.float64, device=q.device)
+
+    def filt(z):
+        p = torch.nn.functional.pad(z, (HALO, HALO, HALO, HALO))
+        h = sum(w[k] * p[:, :, k:k + W] for k in range(len(WINDOW)))
+        return sum(w[k] * h[:, k:k + H, :] for k in range(len(WINDOW)))
+
+    mu1, mu2 = filt(a), filt(b)
+    mu1_sq, mu2_sq, mu1_mu2 = mu1 * mu1, mu2 * mu2, mu1 * mu2
+    s11, s22, s12 = filt(a * a) - mu1_sq, filt(b * b) - mu2_sq, filt(a * b) - mu1_mu2
+    m = ((2 * mu1_mu2 + C1) * (2 * s12 + C2)) / ((mu1_sq + mu2_sq + C1) * (s11 + s22 + C2))
+    d = (q.long() - g.long()) ** 2
+    TY = (H + BLOCK_Y - 1) // BLOCK_Y
+    pad = TY * BLOCK_Y - H
+    m = torch.nn.functional.pad(m, (0, 0, 0, pad)).view(3, TY, BLOCK_Y * W).sum((0, 2))
+    d = torch.nn.functional.pad(d, (0, 0, 0, pad)).view(3, TY, BLOCK_Y * W).sum((0, 2)).double()
+    out = torch.stack([m, d], 1)
+    y0 = torch.arange(TY, device=q.device) * BLOCK_Y
+    out[(y0 < row0) | (torch.clamp(y0 + BLOCK_Y, max=H) > row1)] = 0.0
+    return out
+
+
 def finalize(sl, H, W):
     """(TILE_Y, 2) slots -> (SSIM, PSNR), the rows added in order."""
     s = np.zeros((2,), dtype=np.float64)

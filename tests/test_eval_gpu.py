@@ -81,7 +81,7 @@ def test_slots_against_the_reference(B, H, W):
 def test_nan_inf_and_the_per_channel_psnr():
     H, W = 48, 20
     gt = torch.randint(0, 256, (3, 3, H, W), generator=torch.Generator().manual_seed(1), dtype=torch.uint8)
-    img = gt.float() / 255.0          # view 0: the reference's fp32 gt / 255 exactly -> L1 0, PSNR +inf
+    img = (gt.to(DEV) / 255.0).cpu()  # view 0: the reference's gt / 255.0 on the device exactly -> L1 0, PSNR +inf
     img[1, 2, 30, 7] = float("nan")   # view 1: a diverged pixel -> NaN, in its tile row's slot only
     img[2, 0] += 0.02                 # view 2: channel errors of different size
     img[2, 1] -= 0.2

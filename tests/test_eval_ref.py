@@ -34,6 +34,35 @@ def test_reference_matches_the_reference_formulas(H, W):
     assert got[1] == pytest.approx(want[1], rel=1e-12)
 
 
+def test_ground_truth_unit_is_the_device_product():
+    """gt_hat is fl32(g * fl32(1/255)), which differs from the IEEE quotient, what torch's `/ 255.0` gives on the CPU, on
+    126 byte values, always by one ulp upwards; gt_hat_torch is the same bits on the CPU."""
+    g = np.arange(256, dtype=np.uint8)
+    prod = eval_ref.gt_hat(g).astype(np.float32)
+    quot = (torch.from_numpy(g) / 255.0).numpy()
+    assert np.array_equal(eval_ref.gt_hat_torch(g).numpy().view(np.uint32), prod.view(np.uint32))
+    diff = prod != quot
+    assert int(diff.sum()) == 126
+    assert np.array_equal(prod[diff], np.nextafter(quot[diff], np.float32(2)))
+
+
+@pytest.mark.parametrize("H,W", [(1, 1), (5, 2), (16, 7), (17, 33), (37, 29), (40, 129)])
+def test_torch_slots_match_numpy(H, W):
+    """slots_torch, the large-shape form of slots, against slots at small shapes: NaN, inf, -0, values above 1."""
+    rng = np.random.default_rng(7 * H + W)
+    image = rng.uniform(-0.3, 1.3, size=(3, H, W)).astype(np.float32)
+    gt = rng.integers(0, 256, size=(3, H, W), dtype=np.uint8)
+    flat = image.reshape(-1)
+    flat[:4] = [np.inf, -np.inf, -0.0, 3.0][:flat.size]
+    flat[-1] = np.nan
+    for rows in (None, (0, H), (16, H) if H > 16 else (0, 0), (0, 16) if H > 16 else (0, H)):
+        want = eval_ref.slots(image, gt, rows)
+        got = eval_ref.slots_torch(torch.from_numpy(image), torch.from_numpy(gt), rows).numpy()
+        assert got.shape == want.shape
+        assert np.allclose(got, want, rtol=1e-13, atol=0, equal_nan=True), rows
+        assert np.array_equal(np.signbit(got[want == 0]), np.zeros((want == 0).sum(), bool))
+
+
 def test_psnr_is_per_channel_then_averaged():
     H, W = 32, 16
     gt = np.full((3, H, W), 128, dtype=np.uint8)
@@ -63,7 +92,7 @@ def test_clamp_comes_before_the_comparison():
 
 def test_perfect_image_scores_inf():
     image, gt = _case(24, 40, seed=3)
-    image = eval_ref.gt_hat(gt).astype(np.float32)   # the reference's fp32 gt / 255 exactly
+    image = eval_ref.gt_hat(gt).astype(np.float32)   # the reference's gt / 255.0 on the device exactly
     assert eval_ref.finalize(eval_ref.slots(image, gt), 24, 40) == (0.0, math.inf)
     assert eval_ref.reference_sequence(image, gt, torch.float32) == (0.0, math.inf)
 

@@ -67,6 +67,22 @@ def test_ground_truth_round_trip_is_exact_for_every_value():
     assert np.array_equal(metrics_ref.quantize(saved.numpy()), g)
     back = _png_round_trip(saved)
     assert torch.equal(back, torch.from_numpy(metrics_ref.unit(g).astype(np.float32)))
+    # render.py divides on the device, where the quotient is fl32(g * fl32(1/255)): that comes back as g too
+    import eval_ref
+    assert np.array_equal(metrics_ref.quantize(eval_ref.gt_hat(g).astype(np.float32)), g)
+
+
+@pytest.mark.parametrize("H,W", [(1, 1), (5, 2), (11, 12), (16, 33), (17, 31), (40, 65)])
+def test_torch_slots_match_numpy(H, W):
+    """slots_torch, the large-shape form of slots, against slots at small shapes, whole and strip rows."""
+    rng = np.random.default_rng(H * 100 + W)
+    g = rng.integers(0, 256, (3, H, W), dtype=np.uint8)
+    q = np.clip(g.astype(np.int64) + rng.integers(-9, 10, g.shape), 0, 255).astype(np.uint8)
+    for rows in (None, (16, H) if H > 16 else (0, 0), (0, 16) if H > 16 else (0, H)):
+        want = metrics_ref.slots(q, g, rows)
+        got = metrics_ref.slots_torch(torch.from_numpy(q), torch.from_numpy(g), rows).numpy()
+        assert got.shape == want.shape and np.allclose(got, want, rtol=1e-13, atol=0), rows
+        assert not np.signbit(got[want == 0]).any()
 
 
 def test_window_is_the_reference_gaussian_bit_for_bit():

@@ -137,7 +137,7 @@ def within_ulp(a, b):
 def refs(image, gt_strip, r, gl1, gss):
     """(fp64 reference, fp32 floor, the fp32 floor's summed per-pixel |error| of (Ll1, ssim)) of one view; the first
     two as (Ll1, ssim, grad numpy)."""
-    y = gu.to_dev(lc.gt_float(gu.npy(gt_strip)))          # fl32(gt / 255), as the kernel forms it
+    y = gu.to_dev(lc.gt_float(gu.npy(gt_strip)))          # fl32(gt * fl32(1/255)), as the kernel forms it
     out = []
     for dt in (torch.float64, torch.float32):
         l1, ss, g = loss_ref.strip_loss(image, y, *r, float(gl1), float(gss), dtype=dt)
@@ -247,7 +247,7 @@ L1_SHAPES = [(65, 1), (48, 33), (96, 1920)]
 
 @pytest.mark.parametrize("H,W", L1_SHAPES)
 def test_l1_branch_is_exact(H, W):
-    """grad_ssim = 0: dL/dimage == fl32(fl32(g_l1 * fl32(1 / (3HW))) * sgn(x - fl32(gt / 255))) bit for bit, sgn(0) = 0 and
+    """grad_ssim = 0: dL/dimage == fl32(fl32(g_l1 * fl32(1 / (3HW))) * sgn(x - gt_float(gt))) bit for bit, sgn(0) = 0 and
     0 on halo rows and outside the window; Ll1 within 1e-6 of the exact fp64 sum."""
     rows4 = [(0, H, 0, H), (0, 0, 0, 0), (16, H, 21, H - 5), (H - 33, H, H - 33, H), (3, 19, 10, 10)]
     B = len(rows4)
