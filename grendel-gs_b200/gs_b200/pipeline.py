@@ -152,14 +152,16 @@ class Trainer:
 
     Gaussians are sharded evenly by contiguous chunks (scene/gaussian_model.py:181-194); the B cameras of a
     step are divided into tile-row strips over the W ranks (division.start_strategy); projected splats reach
-    their strip owners through exchange.exchange (skipped when W == 1, like gaussian_renderer/__init__.py:968).
+    their strip owners through exchange.exchange_cat (skipped when W == 1, like gaussian_renderer/__init__.py:968).
+    Every batch renders all its local strips in one batched render (ops.render_gaussians_batched) instead of the
+    reference's per-camera loop (render_final, gaussian_renderer/__init__.py:1217-1288), and scores them in one batched
+    loss (ops.fused_l1_ssim_batched).
     """
 
     def __init__(self, scene, cams, gts_pinned, device, rank=0, world=1, lambda_dssim=0.2, group=None,
-                 fused_activations=True, border_exchange=False, batched_render=True, peer_exchange=None,
-                 peer_cap_rows=None, shard=None, load_balance=True, heuristic_decay=0.0,
-                 distributed_dataset_storage=False, feedback_lag=None, max_sh_degree=3, deterministic=False,
-                 local_sampling=False, local_bsz=None, model=None):
+                 border_exchange=False, peer_exchange=None, peer_cap_rows=None, shard=None, load_balance=True,
+                 heuristic_decay=0.0, distributed_dataset_storage=False, feedback_lag=None, max_sh_degree=3,
+                 deterministic=False, local_sampling=False, local_bsz=None, model=None):
         """cams, gts_pinned: the camera set -- N cameras and their uint8 (3,H,W) host images, all of one size (the reference
         keeps one global TILE_Y); each step trains on the views it lists (step(views=...)), all N by default.
         scene: the WHOLE scene (sliced here into this rank's contiguous shard), or -- shard=(lo, hi, n_total) -- only
@@ -196,7 +198,7 @@ class Trainer:
         self.local_sampling, self.local_bsz = bool(local_sampling), None
         if self.local_sampling:
             self._check_local_sampling(gts_pinned, device, world, group, local_bsz, distributed_dataset_storage,
-                                       fused_activations, batched_render, border_exchange)
+                                       border_exchange)
         if deterministic and world > 1 and load_balance and not self.local_sampling:
             raise ValueError("deterministic=True needs a fixed strip division: pass load_balance=False when world > 1 "
                              "(the load balancer moves the strips by measured times)")
@@ -233,12 +235,8 @@ class Trainer:
             if _dist.get_backend(group) == "nccl":
                 _w = torch.zeros((world,), dtype=torch.float32, device=device)
                 _dist.all_to_all_single(torch.empty_like(_w), _w, group=group)
-        # bin + blend + loss of all B cameras in one pass (ops.render_gaussians_batched) instead of the reference's
-        # per-camera loop (render_final, gaussian_renderer/__init__.py:1217-1288); False keeps the per-camera calls
-        self.batched_render = batched_render
         self.device, self.rank, self.world, self.group = device, rank, world, group
         self.lambda_dssim = lambda_dssim
-        self.fused_activations = fused_activations
         self.border_exchange = border_exchange   # legacy row L1: exchange 5 halo rows so strip losses sum to the full-image loss
         if model is not None:
             self.params = GaussianParams.from_raw(model, device)
@@ -292,9 +290,7 @@ class Trainer:
         self._cam_table_dev = self._cam_rows.to(device) if self.local_sampling else None
         self._whole_views = None   # ((world, rank), the whole-view division of a local-sampling batch)
         self._strategy_cache = None   # ((history version, the batch's camera uids), strategies)
-        self._mask_cache = {}
         self._bmask_cache = {}
-        self._n_renders = 0
         self._copy_stream = None
         self._loss_host = None
         self._local_coef = None    # local sampling: (the loss weights of the local_bsz views, the constant term)
@@ -318,7 +314,7 @@ class Trainer:
         return int(t.item())
 
     def _check_local_sampling(self, gts_pinned, device, world, group, local_bsz, distributed_dataset_storage,
-                              fused_activations, batched_render, border_exchange):
+                              border_exchange):
         """The construction-time refusals of local sampling, before any other collective.  local_bsz and the number of
         images each rank holds are all-gathered first (one small collective, none at world 1) and every rank decides from
         the gathered values, so a rank whose value differs raises together with the others instead of leaving them
@@ -326,9 +322,8 @@ class Trainer:
         if distributed_dataset_storage:
             raise ValueError("local_sampling: every rank holds the images of the views it samples; "
                              "distributed_dataset_storage has no meaning with it")
-        if not fused_activations or not batched_render or border_exchange:
-            raise ValueError("local_sampling runs the fused-activation batched preprocess and render over whole views: "
-                             "fused_activations=False, batched_render=False and border_exchange=True do not apply")
+        if border_exchange:
+            raise ValueError("local_sampling renders and scores whole views: border_exchange=True does not apply")
         try:
             k = operator.index(local_bsz)
         except TypeError:
@@ -545,13 +540,7 @@ class Trainer:
     def _evaluate(self, dcams, host, views, bsz, held_out):
         batches, slots = [], []
         for strategies, rows, gts, gt_row0, fw in self._eval_batches(dcams, host, views, bsz, held_out):
-            if fw.images is not None:
-                s = ops.eval_sums_batched(fw.images, gts, rows, gt_row0)
-            else:   # per-camera renders; the slots of cameras without a strip here stay +0.0
-                s = torch.zeros((len(strategies), self.tile_y, 3, 2), dtype=torch.float64, device=self.device)
-                for k, image, _n in fw.per_camera:
-                    s[k] = ops.eval_sums_batched(image.unsqueeze(0), gts[k:k + 1], rows[k:k + 1], gt_row0[k:k + 1])[0]
-            slots.append(s)
+            slots.append(ops.eval_sums_batched(fw.images, gts, rows, gt_row0))
             batches.append(len(strategies))
         slots = self._sum_slots_over_ranks(torch.cat(slots) if len(slots) > 1 else slots[0])
         per_view, b0 = [], 0
@@ -578,10 +567,7 @@ class Trainer:
                 win = torch.empty((6, b - a, W), dtype=torch.uint8, device=self.device)
                 win[3:, y0 - a:y1 - a].copy_(gts[k][:, y0 - gt_row0[k]:y1 - gt_row0[k]])
                 wins.append(win); win_row0.append(a)
-            if fw.images is not None:
-                ops.quantize_u8_batched(fw.images, rows, [None if w is None else w[:3] for w in wins], win_row0)
-            for k, image, _n in fw.per_camera:
-                ops.quantize_u8_batched(image.unsqueeze(0), rows[k:k + 1], [wins[k][:3]], win_row0[k:k + 1])
+            ops.quantize_u8_batched(fw.images, rows, [None if w is None else w[:3] for w in wins], win_row0)
             if self.world > 1:
                 image_halo.exchange_halos(wins, win_row0, strategies, H, W, self.rank, self.world, self.group, self.device)
             if any(w is not None for w in wins):
@@ -657,52 +643,23 @@ class Trainer:
         k, B, H = self.local_bsz, self.world * self.local_bsz, self.H
         strategies = self._whole_view_division()
         rs = self.dcams[views[0]].settings(p.active_sh_degree)   # image size and background, shared by every view
-        gt_ready = []
-        if not resident:   # the whole own images from pinned host memory, on the copy stream, while the render runs
-            if self._copy_stream is None:
-                self._copy_stream = torch.cuda.Stream(device=self.device)
-            for v in views:
-                with torch.cuda.stream(self._copy_stream):
-                    d = self._strip_h2d(self.gts_host[v], 0, H, cache_key=v)
-                    self._h2d += d.numel()
-                    ev = torch.cuda.Event()
-                    ev.record(self._copy_stream)
-                gt_ready.append((d, ev))
-        if B == 1:   # one view on one rank: the per-camera preprocess, as the default one-view step runs it
-            out = ops.preprocess_gaussians_raw(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation,
-                                               p._opacity, rs)
-            out[0].retain_grad()
-            self.means2D = [out[0]]
-            batched = tuple(t.unsqueeze(0) for t in out)
-        else:
-            batched = ops.preprocess_gaussians_batched(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation,
-                                                       p._opacity, self._gathered_camera_table(views), self.W, self.H,
-                                                       p.active_sh_degree)
-            batched[0].retain_grad()   # (B,P,2): densification reads the screen-space gradients of all B views
-            self.means2D = batched[0]
-        self._radii_local = batched[3]
+        # the whole own images from pinned host memory, on the copy stream, while the render runs
+        gt_ready = [] if resident else [self._copy_gt(v, 0, H) for v in views]
+        batched = self._preprocess(rs, lambda: self._gathered_camera_table(views), B, training=True)
+        self.means2D, self._radii_local = batched[0], batched[3]
         if self.world > 1:
             self._ex.PIGGYBACK_IN = None   # no render times ride on the exchange
             cat, view_start, _cnt = self._ex.exchange_cat(*batched, strategies, [rs], self.world, self.rank, self.group,
                                                           self._peer)
             view_start = view_start[self.rank * k:(self.rank + 1) * k + 1]   # the other views have no rows here
         else:
-            Pn = batched[0].shape[1]
-            cat = (batched[0].reshape(-1, 2), batched[1].reshape(-1, 3), batched[2].reshape(-1, 4),
-                   batched[3].reshape(-1), batched[4].reshape(-1))
-            view_start = [q * Pn for q in range(B + 1)]
+            cat, view_start = self._concat(batched)
         collectors = [{} for _ in range(k)]
         m2, rgb, co, radii, depths = cat
         images, _stats = ops.render_gaussians_batched(m2, co, rgb, depths, radii, None, view_start, rs,
                                                       {"stats_collector": collectors[0]}, deterministic=self.deterministic)
-        if resident:   # the whole resident images, read in place
-            gts = [self.gts_dev[v] for v in views]
-        else:
-            gts = []
-            for gt, ev in gt_ready:
-                torch.cuda.current_stream().wait_event(ev)
-                gt.record_stream(torch.cuda.current_stream())
-                gts.append(gt)
+        # the whole resident images, read in place, or the copies once they have landed
+        gts = [self.gts_dev[v] for v in views] if resident else [self._wait_gt(r) for r in gt_ready]
         if self._local_coef is None:   # the weights and constant the default batched step forms for whole strips
             coef, const = [], 0.0
             for _ in range(k):
@@ -714,7 +671,6 @@ class Trainer:
                                             gt_full=resident)
         loss_sum = torch.dot(l1_ssim.reshape(-1), coef) + const
         loss_sum.backward()
-        self._n_renders = 1
         self._finish_local_step(strategies, collectors, int(view_start[-1]) - int(view_start[0]))
         if resident:
             return None
@@ -759,7 +715,7 @@ class Trainer:
             a.gpu_ids != b.gpu_ids or a.division_pos != b.division_pos for a, b in zip(new, prev[1]))
         self._strategy_cache = ((ver, uids), new)
         if moved and (prev is None or prev[0][0] != ver):   # per-division caches belong to the old boundaries
-            self._strip_cache.clear(); self._mask_cache.clear(); self._bmask_cache.clear()
+            self._strip_cache.clear(); self._bmask_cache.clear()
             self.balance_log.append((self.iteration, [list(st.division_pos) for st in new],
                                      [list(st.gpu_ids) for st in new]))
         return new
@@ -807,68 +763,46 @@ class Trainer:
             ev.record(torch.cuda.current_stream())
             gt_ready = {k: (t, ev) for k, t in strips.items()}
         elif not resident:
-            if self._copy_stream is None:
-                self._copy_stream = torch.cuda.Stream(device=self.device)
+            for k, st in enumerate(strategies):
+                rows = st.local_pixel_rows(self.H)
+                if rows is not None:
+                    gt_ready[k] = self._copy_gt(views[k], rows[0], rows[1])
+        collectors = [{} for _ in dcams]
+        fw = self._forward(settings, strategies, collectors, lambda: self._camera_table(views), training=True)
+        self.means2D, self._radii_local = fw.means2D, fw.radii
+        if self.border_exchange:
+            # the legacy row L1: one loss per local strip, summed in view order; a strip of a view split over several
+            # ranks is widened by the 5 halo rows its neighbours render, so the strip losses sum to the full-image loss
+            loss_sum = None
             for k, st in enumerate(strategies):
                 rows = st.local_pixel_rows(self.H)
                 if rows is None:
                     continue
-                with torch.cuda.stream(self._copy_stream):
-                    d = self._strip_h2d(self.gts_host[views[k]], rows[0], rows[1], cache_key=views[k])
-                    self._h2d += d.numel()
-                    ev = torch.cuda.Event()
-                    ev.record(self._copy_stream)
-                gt_ready[k] = (d, ev)
-        collectors = [{} for _ in dcams]
-        fw = self._forward(settings, strategies, collectors, lambda: self._camera_table(views), training=True)
-        self.means2D, self._radii_local, self._n_renders = fw.means2D, fw.radii, fw.n_renders
-        loss_sum = None
-        Vp = Pl = 0
-        if fw.images is not None:   # one batched render of every local strip
-            rows4, coef, const = fw.rows4, fw.coef, fw.const
-            gts = []
-            for k, (y0, y1, _c0, _c1) in enumerate(rows4):
-                if y1 == y0:
-                    gts.append(None)
-                elif resident:   # the whole resident image, read in place
-                    gts.append(self.gts_dev[views[k]])
+                if len(st.gpu_ids) > 1:
+                    from . import border
+                    image, (r0, r1), _ = border.add_remote_border_rows(fw.images[k], st, self.H, self.group)
+                    loss = ops.fused_loss(image, self.gts_dev[views[k]], r0, r1, self.lambda_dssim, *rows,
+                                          deterministic=self.deterministic, gt_full=True)
                 else:
-                    gt, ev = gt_ready[k]
-                    torch.cuda.current_stream().wait_event(ev)
-                    gt.record_stream(torch.cuda.current_stream())
-                    gts.append(gt)
-            l1_ssim = ops.fused_l1_ssim_batched(fw.images, gts, rows4, deterministic=self.deterministic, gt_full=resident)
+                    gt = self.gts_dev[views[k]] if resident else self._wait_gt(gt_ready[k])
+                    loss = ops.fused_loss(fw.images[k], gt, *rows, self.lambda_dssim, deterministic=self.deterministic,
+                                          gt_full=resident and rows != (0, self.H))
+                loss_sum = loss if loss_sum is None else loss_sum + loss
+        else:
+            gts = [None if y1 == y0 else self.gts_dev[views[k]] if resident else self._wait_gt(gt_ready[k])
+                   for k, (y0, y1, _c0, _c1) in enumerate(fw.rows4)]
+            # the resident image of a one-view batch that is local whole is read as a strip of every row (no host-side
+            # row tables); every other resident image is read in place at its strip rows
+            gt_full = resident and not (len(views) == 1 and fw.rows4[0] == (0, self.H, 0, self.H))
+            l1_ssim = ops.fused_l1_ssim_batched(fw.images, gts, fw.rows4, deterministic=self.deterministic,
+                                                gt_full=gt_full)
             # sum over the local strips of (1 - lambda) Ll1 + lambda (1 - ssim)
-            loss_sum = torch.dot(l1_ssim.reshape(-1), coef) + const
-            Vp = int(fw.view_start[-1])
-            Pl = sum((r[1] - r[0]) * self.W for r in rows4)
-        for k, image, n_splats in fw.per_camera:
-            st = strategies[k]
-            y0, y1 = st.local_pixel_rows(self.H)
-            if self.border_exchange and self.world > 1 and len(st.gpu_ids) > 1:
-                from . import border
-                image, (r0, r1), _ = border.add_remote_border_rows(image, st, self.H, self.group)
-                loss = ops.fused_loss(image, self.gts_dev[views[k]], r0, r1, self.lambda_dssim, y0, y1,
-                                      deterministic=self.deterministic, gt_full=True)
-            else:
-                if resident:
-                    gt = self.gts_dev[views[k]]
-                else:
-                    gt, ev = gt_ready[k]
-                    torch.cuda.current_stream().wait_event(ev)
-                    gt.record_stream(torch.cuda.current_stream())
-                # a strip of every row is the resident image itself: the strip form reads it with no host-side row
-                # tables (the single-rank step); only a part of the image needs the in-place form
-                loss = ops.fused_loss(image, gt, y0, y1, self.lambda_dssim, deterministic=self.deterministic,
-                                      gt_full=resident and (y0, y1) != (0, self.H))
-            loss_sum = loss if loss_sum is None else loss_sum + loss
-            Vp += n_splats
-            Pl += (y1 - y0) * self.W
+            loss_sum = torch.dot(l1_ssim.reshape(-1), fw.coef) + fw.const
         self._mark("r render+loss")
         loss_sum.backward()
         self._mark("b4 backward (rest)")
         self._collectors, self._strategies = collectors, strategies
-        self._counts = dict(Vp=Vp, P_local=Pl)
+        self._counts = dict(Vp=int(fw.view_start[-1]), P_local=sum((r[1] - r[0]) * self.W for r in fw.rows4))
         self.iteration += 1
         self._feed_back_times(strategies, collectors)
         self._mark("t time feedback")
@@ -876,135 +810,108 @@ class Trainer:
             return None
         return self._read_loss(loss_sum)
 
-    def _forward(self, settings, strategies, collectors, cam_table, training):
-        """The forward of one batch, on the path the Trainer's options select: preprocess (all cameras in one batched launch
-        with fused activations, else per camera) -> exchange of the projected splats (W > 1) -> render (one batched render
-        of every local strip, else one render per camera with a strip here).  cam_table(): the (B,40) device camera table
-        of the batched preprocess.  training=False (evaluate): no screen-space gradient is retained and no render times
-        ride on the exchange.
-        -> namespace of means2D and radii (this rank's pre-exchange values, which densification reads); images (B,3,H,W)
-        of the batched render with its rows4 / coef / const / view_start, or None; per_camera [(camera index, image (3,H,W),
-        splats rendered)] of the per-camera renders; n_renders."""
+    def _copy_gt(self, view, y0, y1):
+        """Rows [y0, y1) of a view's host image, copied on the side stream while preprocess / binning / blend run.
+        -> (device strip, the copy's event) for _wait_gt."""
+        if self._copy_stream is None:
+            self._copy_stream = torch.cuda.Stream(device=self.device)
+        with torch.cuda.stream(self._copy_stream):
+            d = self._strip_h2d(self.gts_host[view], y0, y1, cache_key=view)
+            self._h2d += d.numel()
+            ev = torch.cuda.Event()
+            ev.record(self._copy_stream)
+        return d, ev
+
+    @staticmethod
+    def _wait_gt(ready):
+        """The device strip of a (strip, event) pair, once the current stream has waited for its copy."""
+        gt, ev = ready
+        torch.cuda.current_stream().wait_event(ev)
+        gt.record_stream(torch.cuda.current_stream())
+        return gt
+
+    def _preprocess(self, rs, cam_table, B, training):
+        """This rank's Gaussians projected into the B views of a batch -> (means2D (B,P,2), rgb, conic_opacity, radii,
+        depths).  One view runs the per-camera kernel with its settings rs; more run ONE batched launch over the (B,40)
+        device camera table cam_table(), which reads every Gaussian once.  training: means2D keeps its gradient, which
+        densification reads (means2D.grad of camera k, densification.py:24)."""
         p = self.params
-        if not self.fused_activations:  # the reference's five activation kernels + cat (__init__.py:902-906)
-            xyz, scaling, rotation, feats, opacity = p.get_xyz, p.get_scaling, p.get_rotation, p.get_features, p.get_opacity
-        screen = []
-        B = len(settings)
-        use_batched = self.batched_render and B > 1 and not self.border_exchange
-        if self.fused_activations and B > 1:
-            # all B cameras in ONE launch: every Gaussian is read once and projected into each camera
-            bm2, brgb, bco, bradii, bdepths = ops.preprocess_gaussians_batched(
-                p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation, p._opacity, cam_table(),
-                self.W, self.H, p.active_sh_degree)
-            if training:
-                bm2.retain_grad()   # (B,P,2): densification reads bm2.grad[k] (means2D.grad of camera k, densification.py:24)
-            batched = (bm2, brgb, bco, bradii, bdepths)
-            if self.world == 1 and not use_batched:
-                for k in range(B):
-                    screen.append((bm2[k], brgb[k], bco[k], bradii[k], bdepths[k]))
-            settings_loop = []
+        if B == 1:
+            out = tuple(t.unsqueeze(0) for t in ops.preprocess_gaussians_raw(
+                p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation, p._opacity, rs))
         else:
-            batched = None
-            settings_loop = settings
-        for k, rs in enumerate(settings_loop):
-            if self.fused_activations:
-                out = ops.preprocess_gaussians_raw(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation,
-                                                   p._opacity, rs)
-            else:
-                out = ops.preprocess_gaussians(xyz, scaling, rotation, feats, opacity, rs,
-                                               {"stats_collector": collectors[k]})
-            if training:
-                out[0].retain_grad()
-            screen.append(out)
-        means2D = batched[0] if batched is not None else [s[0] for s in screen]
+            out = ops.preprocess_gaussians_batched(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation,
+                                                   p._opacity, cam_table(), self.W, self.H, p.active_sh_degree)
+        if training:
+            out[0].retain_grad()
+        return out
+
+    @staticmethod
+    def _concat(batched):
+        """On one rank the (B,P,.) projections ARE the concatenation of the views' splats: camera k = rows [k P, (k+1) P).
+        -> (concatenated tensors, view_start)."""
+        B, Pn = batched[0].shape[:2]
+        return tuple(t.reshape(B * Pn, *t.shape[2:]) for t in batched), [k * Pn for k in range(B + 1)]
+
+    def _forward(self, settings, strategies, collectors, cam_table, training):
+        """The forward of one batch: preprocess (_preprocess) -> exchange of the projected splats (exchange_cat, W > 1) or
+        their concatenation (W == 1) -> one batched render of every local strip.  cam_table(): the (B,40) device camera
+        table of the batched preprocess.  training=False (evaluate): no screen-space gradient is retained and no render
+        times ride on the exchange.
+        -> namespace of means2D (B,P,2) and radii (B,P) (this rank's pre-exchange values, which densification reads),
+        images (B,3,H,W), the local strips' rows4 and loss weights coef / const, and view_start."""
+        B = len(settings)
+        batched = self._preprocess(settings[0], cam_table, B, training)
         self._mark("p preprocess")
-        if batched is None and (self.world > 1 or use_batched):
-            # per-camera results (B == 1 or unfused activations): stack into (B,P,.)
-            batched = tuple(torch.stack([s[q] for s in screen]) for q in range(5))
-        cat = view_start = None
         if self.world > 1:
             if training:
                 self._feedback_before_exchange()
             else:
                 self._ex.PIGGYBACK_IN = None
-            if use_batched:
-                cat, view_start, cnt = self._ex.exchange_cat(*batched, strategies, settings, self.world, self.rank,
-                                                             self.group, self._peer)
-            else:
-                redistributed, cnt = self._ex.exchange(*batched, strategies, settings, self.world, self.rank, self.group,
-                                                       self._peer)
+            cat, view_start, _cnt = self._ex.exchange_cat(*batched, strategies, settings, self.world, self.rank,
+                                                          self.group, self._peer)
             if training:
                 self._feedback_after_exchange()
-        elif use_batched:   # (B,P,.) stacked IS the concatenation: camera k = rows [k P, (k+1) P)
-            Pn = batched[0].shape[1]
-            cat = (batched[0].reshape(-1, 2), batched[1].reshape(-1, 3), batched[2].reshape(-1, 4),
-                   batched[3].reshape(-1), batched[4].reshape(-1))
-            view_start = [k * Pn for k in range(B + 1)]
         else:
-            redistributed = screen
-        radii = (batched[3] if batched is not None else
-                 screen[0][3].unsqueeze(0) if len(screen) == 1 else torch.stack([s[3] for s in screen]))
+            cat, view_start = self._concat(batched)
         self._mark("x5 unpack")
-        fw = SimpleNamespace(means2D=means2D, radii=radii, images=None, view_start=view_start, per_camera=[],
-                             n_renders=0)
-        if use_batched:
-            mk = tuple((tuple(st.gpu_ids), tuple(st.division_pos), st.rank) for st in strategies)
-            if mk not in self._bmask_cache:
-                m = torch.zeros((B, self.tile_y, self.tile_x), dtype=torch.uint8, device=self.device)
-                rows4, coef, const = [], [], 0.0
-                for k, st in enumerate(strategies):
-                    r = st.local_rows()
-                    if r is None:   # no strip of this camera here: no tiles, no loss term
-                        rows4.append((0, 0, 0, 0))
-                        coef += [0.0, 0.0]
-                        continue
-                    m[k, r[0]:r[1]] = 1
-                    y0, y1 = st.local_pixel_rows(self.H)
-                    rows4.append((y0, y1, y0, y1))
-                    coef += [1.0 - self.lambda_dssim, -self.lambda_dssim]
-                    const += self.lambda_dssim
-                self._bmask_cache[mk] = (m.reshape(B, -1), rows4,
-                                         torch.tensor(coef, dtype=torch.float32, device=self.device), const)
-            cl, fw.rows4, fw.coef, fw.const = self._bmask_cache[mk]
-            m2, rgb, co, radii, depths = cat
-            fw.images, _stats = ops.render_gaussians_batched(m2, co, rgb, depths, radii, cl, view_start, settings[0],
-                                                             {"stats_collector": collectors[0]},
-                                                             deterministic=self.deterministic)
-            fw.n_renders = 1
-            return fw
-        for k, st in enumerate(strategies):
-            rows = st.local_rows()
-            if rows is None:
-                continue
-            fw.n_renders += 1
-            m2, rgb, co, radii, depths = redistributed[k]
-            ck = (tuple(st.gpu_ids), tuple(st.division_pos), st.rank)
-            if ck not in self._mask_cache:
-                self._mask_cache[ck] = st.get_compute_locally(self.tile_x, self.device)
-            cl = self._mask_cache[ck]
-            image, *_ = ops.render_gaussians(m2, co, rgb, depths, radii, cl, settings[k],
-                                             {"stats_collector": collectors[k]}, deterministic=self.deterministic)
-            fw.per_camera.append((k, image, m2.shape[0]))
-        return fw
+        mk = tuple((tuple(st.gpu_ids), tuple(st.division_pos), st.rank) for st in strategies)
+        if mk not in self._bmask_cache:
+            m = torch.zeros((B, self.tile_y, self.tile_x), dtype=torch.uint8, device=self.device)
+            rows4, coef, const = [], [], 0.0
+            for k, st in enumerate(strategies):
+                r = st.local_rows()
+                if r is None:   # no strip of this camera here: no tiles, no loss term
+                    rows4.append((0, 0, 0, 0))
+                    coef += [0.0, 0.0]
+                    continue
+                m[k, r[0]:r[1]] = 1
+                y0, y1 = st.local_pixel_rows(self.H)
+                rows4.append((y0, y1, y0, y1))
+                coef += [1.0 - self.lambda_dssim, -self.lambda_dssim]
+                const += self.lambda_dssim
+            self._bmask_cache[mk] = (m.reshape(B, -1), rows4,
+                                     torch.tensor(coef, dtype=torch.float32, device=self.device), const)
+        cl, rows4, coef, const = self._bmask_cache[mk]
+        m2, rgb, co, radii, depths = cat
+        images, _stats = ops.render_gaussians_batched(m2, co, rgb, depths, radii, cl, view_start, settings[0],
+                                                      {"stats_collector": collectors[0]}, deterministic=self.deterministic)
+        return SimpleNamespace(means2D=batched[0], radii=batched[3], images=images, rows4=rows4, coef=coef, const=const,
+                               view_start=view_start)
 
-    def _times_of(self, strategies, collectors, n_renders):
-        """This rank's gpu_camera_running_time row for one step: the render time of each camera it rendered a strip of."""
+    def _times_of(self, strategies, collectors):
+        """This rank's gpu_camera_running_time row for one step: the render time of each camera it rendered a strip of.
+        One batched render served all local strips; with several, its time is apportioned by strip height (the
+        reference times every camera's render separately, render_final __init__.py:1217-1288)."""
         from .division import running_time_of
-        B = len(strategies)
-        mine = [-1.0] * B
+        mine = [-1.0] * len(strategies)
         rows = [(st.local_rows()[1] - st.local_rows()[0]) if st.local_rows() is not None else 0 for st in strategies]
-        if n_renders == 1 and sum(1 for r in rows if r) > 1:
-            # one batched render served all local strips: its time is apportioned by strip height (the reference times
-            # every camera's render separately, render_final __init__.py:1217-1288)
+        n_local = sum(1 for r in rows if r)
+        if n_local:
             t = running_time_of(collectors[0])
             for k, r in enumerate(rows):
                 if r:
-                    mine[k] = t * r / sum(rows)
-        else:
-            for k, r in enumerate(rows):
-                if r:
-                    c = collectors[k] if "forward_render_time" in collectors[k] else collectors[0]
-                    mine[k] = running_time_of(c)
+                    mine[k] = t if n_local == 1 else t * r / sum(rows)
         return mine
 
     def _feedback_before_exchange(self):
@@ -1013,13 +920,13 @@ class Trainer:
         self._ex.PIGGYBACK_IN, self._sent_feedback = None, None
         if self.feedback_lag > 0 and len(self._pending_feedback) >= self.feedback_lag:
             entry = self._pending_feedback.pop(0)
-            self._ex.PIGGYBACK_IN = self._times_of(entry[0], entry[1], entry[3])
+            self._ex.PIGGYBACK_IN = self._times_of(entry[0], entry[1])
             self._sent_feedback = entry
 
     def _feedback_after_exchange(self):
         if self._sent_feedback is None:
             return
-        strategies, _collectors, iteration, _n = self._sent_feedback
+        strategies, _collectors, iteration = self._sent_feedback
         times = self._ex.PIGGYBACK_OUT
         self._ex.PIGGYBACK_IN, self._sent_feedback = None, None
         if times is not None:
@@ -1038,9 +945,9 @@ class Trainer:
             self._pending_feedback.clear()
             return
         if self.feedback_lag > 0:   # fed back later, on the size all-gather of a coming exchange (_feedback_before_exchange)
-            self._pending_feedback.append((strategies, collectors, self.iteration, self._n_renders))
+            self._pending_feedback.append((strategies, collectors, self.iteration))
             return
-        mine = self._times_of(strategies, collectors, self._n_renders)
+        mine = self._times_of(strategies, collectors)
         loc = torch.tensor(mine, dtype=torch.float32, device=self.device)
         allt = torch.empty((self.world * B,), dtype=torch.float32, device=self.device)
         dist.all_gather_into_tensor(allt, loc, group=self.group)
@@ -1050,11 +957,10 @@ class Trainer:
     def add_densification_stats(self, xyz_gradient_accum, denom, max_radii2D):
         """The densification statistics of the last step (densification.py:15-24), in place, one launch, no host sync:
         densify.add_densification_stats over this rank's screen-space gradients and pre-exchange radii of every camera of
-        the step (the reference's batched_locally_preprocessed_mean2D / _radii), whichever of the batched or per-camera
-        preprocess the step ran.  xyz_gradient_accum, denom: (P, 1), max_radii2D: (P,), float32, P = n_local."""
+        the step (the reference's batched_locally_preprocessed_mean2D / _radii).  xyz_gradient_accum, denom: (P, 1),
+        max_radii2D: (P,), float32, P = n_local."""
         from . import densify
-        grads = self.means2D.grad if isinstance(self.means2D, torch.Tensor) else [m.grad for m in self.means2D]
-        densify.add_densification_stats(xyz_gradient_accum, denom, max_radii2D, grads, self._radii_local)
+        densify.add_densification_stats(xyz_gradient_accum, denom, max_radii2D, self.means2D.grad, self._radii_local)
 
     GROUP_OF = {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity",
                 "scaling": "_scaling", "rotation": "_rotation"}
@@ -1079,5 +985,5 @@ class Trainer:
 
     def io_bytes_per_step(self):
         """(host->device, device->host) bytes of the last resident=False step: GT strips in, loss out
-        (+ the 8-byte instance count each render reads back)."""
-        return int(self._h2d), 4 + 8 * self._n_renders
+        (+ the 8-byte instance count the step's one render reads back)."""
+        return int(self._h2d), 4 + 8

@@ -38,17 +38,14 @@ class SimRanks:
             exchange.PIGGYBACK_OUT = None if ins[0] is None else np.asarray(ins, dtype=np.float32)
             tr._feedback_after_exchange()
         exchange.PIGGYBACK_IN = exchange.PIGGYBACK_OUT = None
-        times = [[-1.0] * len(views) for _ in self.trs]
+        times = []
         for r, (tr, sts) in enumerate(zip(self.trs, strategies)):
+            # one batched render per rank: its time is the sum over the rank's strips, in collectors[0]
+            t = sum(float(render_times(r, k, st)) for k, st in enumerate(sts) if st.local_rows() is not None)
             collectors = [{} for _ in sts]
-            n = 0
-            for k, st in enumerate(sts):
-                if st.local_rows() is not None:
-                    t = float(np.float32(render_times(r, k, st)))
-                    times[r][k] = t
-                    collectors[k] = {"forward_render_time": t, "backward_render_time": 0.0}
-                    n += 1
-            tr._n_renders = n
+            collectors[0] = {"forward_render_time": t, "backward_render_time": 0.0}
+            # the times the rank feeds back, as the float32 all-gather carries them
+            times.append([float(np.float32(x)) for x in tr._times_of(sts, collectors)])
             tr.iteration += 1
             tr._feed_back_times(sts, collectors)
         self.log.append((strategies[0], times))

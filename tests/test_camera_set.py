@@ -61,9 +61,9 @@ def test_strategy_cache_is_keyed_by_uids():
     b = tr._batch_strategies((41, 40))
     assert b is not a and [s.camera_uid for s in b] == [41, 40]
     masks = {("geometry",): 1}
-    tr._mask_cache.update(masks)
+    tr._bmask_cache.update(masks)
     tr._batch_strategies((45,))                               # another batch: the division-keyed caches stay
-    assert tr._mask_cache == masks and len(tr.balance_log) == 1
+    assert tr._bmask_cache == masks and len(tr.balance_log) == 1
 
 
 @pytest.mark.parametrize("lag", [2, 1])

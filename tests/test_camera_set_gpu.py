@@ -37,8 +37,8 @@ def camera_set():
     return scene, cams, gts
 
 
-def trainer(scene, cams, gts, fused=True):
-    return pipeline.Trainer(scene, cams, gts, DEV, fused_activations=fused, batched_render=fused, deterministic=True)
+def trainer(scene, cams, gts):
+    return pipeline.Trainer(scene, cams, gts, DEV, deterministic=True)
 
 
 def grads_of(tr):
@@ -48,26 +48,24 @@ def grads_of(tr):
 def assert_same_step(a, b, what):
     for k, (x, y) in enumerate(zip(grads_of(a), grads_of(b))):
         assert same_bits(x, y), f"{what}: gradient of parameter {k} differs"
-    ga = a.means2D.grad if isinstance(a.means2D, torch.Tensor) else torch.stack([m.grad for m in a.means2D])
-    gb = b.means2D.grad if isinstance(b.means2D, torch.Tensor) else torch.stack([m.grad for m in b.means2D])
-    assert same_bits(ga, gb), f"{what}: screen-space gradients differ"
+    assert same_bits(a.means2D.grad, b.means2D.grad), f"{what}: screen-space gradients differ"
 
 
-# (a) a batch of a camera set is the Trainer of exactly those cameras
-@pytest.mark.parametrize("path", ["batched", "per_camera"])
+# (a) a batch of a camera set is the Trainer of exactly those cameras; a batch of one view runs the per-camera preprocess
+@pytest.mark.parametrize("path", ["batched", "one_view"])
 @pytest.mark.parametrize("resident", [True, False])
 def test_views_equal_trainer_on_those_cameras(camera_set, path, resident):
     scene, cams, gts = camera_set
-    fused = path == "batched"
-    whole = trainer(scene, cams, gts, fused)
-    sub = trainer(scene, [cams[i] for i in VIEWS], [gts[i] for i in VIEWS], fused)
-    la = whole.step(views=VIEWS, resident=resident)
+    views = VIEWS if path == "batched" else VIEWS[:1]
+    whole = trainer(scene, cams, gts)
+    sub = trainer(scene, [cams[i] for i in views], [gts[i] for i in views])
+    la = whole.step(views=views, resident=resident)
     lb = sub.step(resident=resident)
     if not resident:
         assert np.float32(la).view(np.int32) == np.float32(lb).view(np.int32), (la, lb)
     assert_same_step(whole, sub, f"{path}, resident={resident}")
-    # one view: the per-camera path of the batched preprocess, too
-    one = trainer(scene, [cams[5]], [gts[5]], fused)
+    # one view after a batch: the per-camera preprocess, too
+    one = trainer(scene, [cams[5]], [gts[5]])
     whole.step(views=[5], resident=resident)
     one.step(resident=resident)
     assert_same_step(whole, one, f"{path}, one view")

@@ -281,31 +281,31 @@ def test_no_host_sync():
     assert n >= B
 
 
-# (f) end to end: Trainer steps, then densify_and_prune
-@pytest.mark.parametrize("path", ["batched", "per_camera"])
+# (f) end to end: Trainer steps, then densify_and_prune; "one_view" steps through the views one at a time, which runs the
+# per-camera preprocess
+@pytest.mark.parametrize("path", ["batched", "one_view"])
 def test_trainer_statistics_and_densification(path):
     cfg = syn.CONFIGS["c1"]
     W, H, N, B = cfg["width"], cfg["height"], cfg["n"], 4
     scene = syn.make_scene(N, W, H, seed=0)
     cams = syn.make_batch_cameras(W, H, B)
     gts = [torch.from_numpy(syn.make_gt_image(W, H, seed=1 + k)).pin_memory() for k in range(B)]
-    fused = path == "batched"
+    batches = [None] * 4 if path == "batched" else [[k] for k in range(B)] * 4
     runs = {}
     for way in ("kernel", "reference"):
-        tr = pipeline.Trainer(scene, cams, gts, torch.device("cuda", 0), fused_activations=fused, batched_render=fused,
-                              deterministic=True)
+        tr = pipeline.Trainer(scene, cams, gts, torch.device("cuda", 0), deterministic=True)
         opt = FusedAdam(tr.optimizer_groups(), lr=0.0, eps=1e-15)
         P = tr.n_local
         st = (torch.zeros((P, 1), device=DEV), torch.zeros((P, 1), device=DEV), torch.zeros((P,), device=DEV))
-        for _ in range(4):
-            tr.step(resident=True)
-            assert isinstance(tr.means2D, torch.Tensor) == fused
+        for views in batches:
+            tr.step(views=views, resident=True)
+            nv = B if views is None else len(views)
+            assert isinstance(tr.means2D, torch.Tensor) and tuple(tr.means2D.shape) == (nv, P, 2)
             if way == "kernel":
                 tr.add_densification_stats(*st)
             else:
-                grads = tr.means2D.grad.unbind(0) if fused else [m.grad for m in tr.means2D]
-                reference_chain(*st, grads, tr._radii_local.unbind(0))
-            opt.step(grad_scale=1.0 / B)
+                reference_chain(*st, tr.means2D.grad.unbind(0), tr._radii_local.unbind(0))
+            opt.step(grad_scale=1.0 / nv)
         runs[way] = (tr, opt, st)
     assert_equal_stats(runs["kernel"][2], runs["reference"][2], path)
     accum, denom, maxr = runs["kernel"][2]

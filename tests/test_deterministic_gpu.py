@@ -219,17 +219,16 @@ SCHEDULE = (0, 0, 1, 2, 3, 3)
 DENSIFY_AFTER = 3
 
 
-def training_run(sc, D_max, fused, noise, top):
+def training_run(sc, D_max, one_view, noise, top):
     cams = [pc.golden_camera(5, TW, TH, uid=0), pc.golden_camera(4, TW, TH, uid=1)]
     gts = [torch.from_numpy(pc.syn.make_gt_image(TW, TH, seed=5 + k)).pin_memory() for k in range(2)]
-    tr = pipeline.Trainer(sc, cams, gts, torch.device("cuda", 0), fused_activations=fused, batched_render=fused,
-                          max_sh_degree=D_max, deterministic=True)
+    tr = pipeline.Trainer(sc, cams, gts, torch.device("cuda", 0), max_sh_degree=D_max, deterministic=True)
     opt = FusedAdam(tr.optimizer_groups(), lr=0.0, eps=1e-15)
     losses, counts = [], None
     for it, deg in enumerate(SCHEDULE):
         tr.params.active_sh_degree = min(deg, top)
-        losses.append(tr.step(resident=False))
-        opt.step(grad_scale=0.5)
+        losses.append(tr.step(views=[it % 2] if one_view else None, resident=False))
+        opt.step(grad_scale=1.0 if one_view else 0.5)
         if it == DENSIFY_AFTER:       # statistics and thresholds from this run's own gradients
             p = tr.params
             accum = p._xyz.grad.norm(dim=1, keepdim=True)
@@ -255,8 +254,8 @@ def _scene(seed):
 def test_training_run_is_bit_identical_twice():
     sc = _scene(91)
     noise = torch.randn((2 * 30000, 3), generator=torch.Generator().manual_seed(5)).to(gu.DEV)
-    l1, c1, s1 = training_run(sc, 3, True, noise, 3)
-    l2, c2_, s2 = training_run(sc, 3, True, noise, 3)
+    l1, c1, s1 = training_run(sc, 3, False, noise, 3)
+    l2, c2_, s2 = training_run(sc, 3, False, noise, 3)
     print(f"[det] losses {l1}")
     assert l1 == l2 and c1 == c2_ and c1[1] > 0 and c1[3] > 0
     for name in s1:
@@ -264,9 +263,9 @@ def test_training_run_is_bit_identical_twice():
             assert bits_equal(s1[name][q], s2[name][q]), (name, q)
 
 
-@pytest.mark.parametrize("fused", [True, False], ids=["fused_batched", "plain_dropin"])
+@pytest.mark.parametrize("one_view", [False, True], ids=["fused_batched", "one_view"])
 @pytest.mark.parametrize("D_max", [0, 1, 2])
-def test_training_run_equals_the_padded_run_bit_for_bit(D_max, fused):
+def test_training_run_equals_the_padded_run_bit_for_bit(D_max, one_view):
     """What test_sh_storage_gpu.test_training_run_equals_the_padded_run checks to a tolerance, with deterministic=True
     bit for bit over all six steps: losses, densify counts, parameters and both Adam moments."""
     K = (D_max + 1) ** 2
@@ -275,8 +274,8 @@ def test_training_run_equals_the_padded_run_bit_for_bit(D_max, fused):
     padded["shs"][:, K:] = 0.0
     stored = dict(padded, shs=np.ascontiguousarray(padded["shs"][:, :K]))
     noise = torch.randn((2 * 30000, 3), generator=torch.Generator().manual_seed(D_max)).to(gu.DEV)
-    lK, cK, sK = training_run(stored, D_max, fused, noise, D_max)
-    l16, c16, s16 = training_run(padded, 3, fused, noise, D_max)
+    lK, cK, sK = training_run(stored, D_max, one_view, noise, D_max)
+    l16, c16, s16 = training_run(padded, 3, one_view, noise, D_max)
     assert lK == l16, (lK, l16)
     assert cK == c16 and cK[1] > 0 and cK[3] > 0
     for name in sK:

@@ -536,22 +536,33 @@ def test_batched_render_and_loss_equal_per_camera():
 
 
 def test_trainer_batched_render_equals_per_camera_loop():
-    """Trainer.step with the batched render/loss path against the per-camera loop: same loss, same parameter gradients."""
-    from gs_b200 import pipeline
+    """Trainer.step (one batched preprocess, render and loss) against a loop of the per-camera operators: same loss, same
+    parameter gradients, same screen-space gradients."""
+    from gs_b200 import ops, pipeline
     W, H, n, B = 320, 208, 25000, 3
     sc = syn.make_scene(n, W, H, seed=77, radius_px=8.0)
     cams = syn.make_batch_cameras(W, H, B)
     gts = [torch.from_numpy(syn.make_gt_image(W, H, seed=80 + k)).pin_memory() for k in range(B)]
-    res = []
-    for batched in (False, True):
-        tr = pipeline.Trainer(sc, cams, gts, torch.device("cuda"), batched_render=batched)
-        loss = tr.step(resident=False)
-        res.append((loss, [t.grad.clone() for t in tr.params.raw_parameters()], tr.means2D.grad.clone(), tr.io_bytes_per_step()))
-    assert abs(res[0][0] - res[1][0]) <= 2e-6 * abs(res[0][0])
-    for a, b, name in zip(res[1][1], res[0][1], ("xyz", "f_dc", "f_rest", "scaling", "rotation", "opacity")):
-        _grad_close(a, b, name)
-    _grad_close(res[1][2], res[0][2], "means2D.grad (densification statistic)")
-    assert res[0][3][0] == res[1][3][0] and res[1][3][1] < res[0][3][1]   # same GT bytes in, one count read back, not B
+    params = pipeline.GaussianParams(sc, "cuda")
+    loss, m2s = None, []
+    for k, cam in enumerate(cams):
+        rs = pipeline.DeviceCamera(cam, "cuda").settings(params.active_sh_degree)
+        m2, rgb, co, radii, depths = ops.preprocess_gaussians_raw(params._xyz, params._features_dc, params._features_rest,
+                                                                  params._scaling, params._rotation, params._opacity, rs)
+        m2.retain_grad()
+        m2s.append(m2)
+        image, *_ = ops.render_gaussians(m2, co, rgb, depths, radii, None, rs)
+        lk = ops.fused_loss(image, gts[k].cuda(), 0, H, 0.2)
+        loss = lk if loss is None else loss + lk
+    loss.backward()
+    tr = pipeline.Trainer(sc, cams, gts, torch.device("cuda"))
+    got = tr.step(resident=False)
+    assert abs(got - float(loss)) <= 2e-6 * abs(float(loss))
+    for a, p, name in zip(tr.params.raw_parameters(), params.raw_parameters(),
+                          ("xyz", "f_dc", "f_rest", "scaling", "rotation", "opacity")):
+        _grad_close(a.grad, p.grad, name)
+    _grad_close(tr.means2D.grad, torch.stack([m.grad for m in m2s]), "means2D.grad (densification statistic)")
+    assert tr.io_bytes_per_step() == (B * 3 * H * W, 12)   # the GT images in; the loss and ONE count read back, not B
 
 
 def test_c2_scale_step_against_the_oracle(o32):

@@ -99,7 +99,6 @@ def test_refusals_before_any_collective_or_launch(no_collective_or_launch):
     gts = images_held(6, 1, 0)
     bad_args = [dict(local_bsz=None), dict(local_bsz=0), dict(local_bsz=-2), dict(local_bsz=1.5), dict(local_bsz="2"),
                 dict(local_bsz=65), dict(local_bsz=2, distributed_dataset_storage=True),
-                dict(local_bsz=2, fused_activations=False), dict(local_bsz=2, batched_render=False),
                 dict(local_bsz=2, border_exchange=True)]
     for kw in bad_args:
         with pytest.raises(ValueError):

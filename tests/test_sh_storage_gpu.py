@@ -259,17 +259,16 @@ SCHEDULE = (0, 0, 1, 2, 3, 3)          # active degree per step (capped at the s
 DENSIFY_AFTER = 3
 
 
-def _training_run(sc, D_max, fused, noise, top, shared=None):
+def _training_run(sc, D_max, one_view, noise, top, shared=None):
     cams = [pc.golden_camera(5, TW, TH, uid=0), pc.golden_camera(4, TW, TH, uid=1)]
     gts = [torch.from_numpy(pc.syn.make_gt_image(TW, TH, seed=5 + k)).pin_memory() for k in range(2)]
-    tr = pipeline.Trainer(sc, cams, gts, torch.device("cuda", 0), fused_activations=fused, batched_render=fused,
-                          max_sh_degree=D_max)
+    tr = pipeline.Trainer(sc, cams, gts, torch.device("cuda", 0), max_sh_degree=D_max)
     opt = FusedAdam(tr.optimizer_groups(), lr=0.0, eps=1e-15)
     losses, counts = [], None
     for it, deg in enumerate(SCHEDULE):
         tr.params.active_sh_degree = min(deg, top)
-        losses.append(tr.step(resident=False))
-        opt.step(grad_scale=0.5)
+        losses.append(tr.step(views=[it % 2] if one_view else None, resident=False))
+        opt.step(grad_scale=1.0 if one_view else 0.5)
         if it == DENSIFY_AFTER:
             p = tr.params
             if shared is None:     # the statistics and thresholds of the first run, handed to the second
@@ -289,9 +288,9 @@ def _training_run(sc, D_max, fused, noise, top, shared=None):
     return losses, counts, state, shared
 
 
-@pytest.mark.parametrize("fused", [True, False], ids=["fused_batched", "plain_dropin"])
+@pytest.mark.parametrize("one_view", [False, True], ids=["fused_batched", "one_view"])
 @pytest.mark.parametrize("D_max", [0, 1, 2])
-def test_training_run_equals_the_padded_run(D_max, fused):
+def test_training_run_equals_the_padded_run(D_max, one_view):
     """Six Trainer.steps over two posed cameras with FusedAdam, the active degree raised 0 -> D_max, one
     densify_and_prune (clones and splits, the same noise and statistics) after the fourth, the K-coefficient model against
     the padded degree-3 model.  The first step's loss is bit-identical (preprocess, binning, blend and loss forward are
@@ -299,8 +298,7 @@ def test_training_run_equals_the_padded_run(D_max, fused):
     (test_gpu_parity.test_block_cull_is_invisible), so two runs of even the same model differ in the last bits: the
     later losses agree to 1e-5 relative, parameters and moments under test_gpu_parity's bar (1e-4 relative + 1e-4 x
     RMS, all but 1e-3 of the entries), densify counts exactly.  The padded coefficients and their moments stay exactly 0.
-    fused: fused activations + batched preprocess / render; otherwise the reference's activations, get_features and the
-    per-camera drop-in operators."""
+    one_view: each step trains one of the two views (the per-camera preprocess) instead of both in one batch."""
     K = _K(D_max)
     cam = pc.golden_camera(5, TW, TH)
     sc, _ = pc.region_scene(cam, 30000, seed=77 + D_max, mix=pc.MILD)
@@ -308,10 +306,10 @@ def test_training_run_equals_the_padded_run(D_max, fused):
     padded["shs"][:, K:] = 0.0
     stored = dict(padded, shs=np.ascontiguousarray(padded["shs"][:, :K]))
     noise = torch.randn((2 * 30000, 3), generator=torch.Generator().manual_seed(D_max)).to(gu.DEV)
-    lK, cK, sK, shared = _training_run(stored, D_max, fused, noise, D_max)
-    l16, c16, s16, _ = _training_run(padded, 3, fused, noise, D_max, shared)
+    lK, cK, sK, shared = _training_run(stored, D_max, one_view, noise, D_max)
+    l16, c16, s16, _ = _training_run(padded, 3, one_view, noise, D_max, shared)
     same = all(bits_equal(sK[n][q], s16[n][q][:, :K - 1] if n == "f_rest" else s16[n][q]) for n in sK for q in range(3))
-    print(f"[sh-storage] D_max {D_max} fused={fused}: losses {lK} vs padded {l16}; densify counts {cK}; parameters and "
+    print(f"[sh-storage] D_max {D_max} one_view={one_view}: losses {lK} vs padded {l16}; densify counts {cK}; parameters and "
           f"moments bit-identical: {same}")
     assert lK[0] == l16[0]
     np.testing.assert_allclose(lK, l16, rtol=1e-5, atol=0)
