@@ -25,12 +25,12 @@ from . import _lib, ops
 ROW, GROW = 11, 9
 MAX_CAMERAS, MAX_RANKS, MAX_SEGMENTS = 16, 16, 128   # XB, XW, XSEG of csrc/distribute.cu
 MODE = "direct"   # the exchange over peer memory: direct placement (bench.py reports it)
-TRACE = None   # diagnostics: callable(name) that synchronises and charges the time since the last mark (pipeline._mark)
 
 
-def _t(name):
-    if TRACE is not None:
-        TRACE(name)
+def _t(mark, name):
+    """Diagnostics: mark(name) synchronises and charges the time since the last mark (pipeline.Trainer._mark)."""
+    if mark is not None:
+        mark(name)
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -99,35 +99,32 @@ def all_to_all_single(out, inp, out_splits, in_splits, group=None):
 
 # Timing feedback rides on the exchange: the render times a rank wants to share (a few floats, finish_strategy_final's
 # all-gather of utils/general_utils.py:249-269) are all-gathered right behind the sizes and read back with them -- no
-# collective of their own on the critical path, no extra host sync.  The caller (pipeline.Trainer) sets PIGGYBACK_IN to a
-# list of floats before the exchange (None on steps without feedback: the same on every rank) and reads PIGGYBACK_OUT, a
-# (W, len) array, afterwards.
-PIGGYBACK_IN = None
-PIGGYBACK_OUT = None
+# collective of their own on the critical path, no extra host sync.  The caller (pipeline.Trainer) passes them as `times`,
+# a list of floats (None on steps without feedback, on every rank alike: then no all-gather is issued), and gets every
+# rank's list back as a (W, len) float32 array.
 _WARNED_OVER_CAPACITY = False
 
 
-def _piggyback_gather(dev, world, group):
-    """Enqueue the all-gather of PIGGYBACK_IN (if any) on the current stream -> device tensor (W * E) or None."""
-    if PIGGYBACK_IN is None:
+def _gather_times(times, dev, world, group):
+    """Enqueue the all-gather of `times` (if any) on the current stream -> device tensor (W * E) or None."""
+    if times is None:
         return None
-    mine = torch.tensor([float(v) for v in PIGGYBACK_IN], dtype=torch.float32, device=dev)
+    mine = torch.tensor([float(v) for v in times], dtype=torch.float32, device=dev)
     allp = torch.empty((world * mine.numel(),), dtype=torch.float32, device=dev)
     dist.all_gather_into_tensor(allp, mine, group=group)
     return allp
 
 
-def gather_counts(local_counts, group=None):
-    """(B, W) int32 device tensor -> (W, B, W) integer array cnt[i][k][j]; the step's one host sync."""
-    global PIGGYBACK_OUT
+def gather_counts(local_counts, group=None, times=None):
+    """(B, W) int32 device tensor -> ((W, B, W) integer array cnt[i][k][j], every rank's `times` as a (W, len) float32
+    array or None without times); the step's one host sync."""
     W = dist.get_world_size(group)
     flat = local_counts.contiguous().reshape(-1)
     allc = torch.empty((W * flat.numel(),), dtype=flat.dtype, device=flat.device)
     dist.all_gather_into_tensor(allc, flat, group=group)
-    allp = _piggyback_gather(flat.device, W, group)
+    allp = _gather_times(times, flat.device, W, group)
     out = allc.reshape((W,) + tuple(local_counts.shape)).cpu().numpy()
-    PIGGYBACK_OUT = None if allp is None else allp.reshape(W, -1).cpu().numpy()
-    return out
+    return out, None if allp is None else allp.reshape(W, -1).cpu().numpy()
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -306,11 +303,11 @@ class _ExchangeSplats(torch.autograd.Function):
         send = torch.empty((max(layout.total_send, 1), ROW), dtype=torch.float32, device=dev)
         _lib.call("gs_xchg_pack", B, P, W, state["flags"].data_ptr(), state["gpos"].data_ptr(), _slab_ptrs(m2, B),
                   _slab_ptrs(rgb, B), _slab_ptrs(co, B), _slab_ptrs(radii, B), _slab_ptrs(depths, B), send.data_ptr(), s)
-        _t("x3 pack")
+        _t(state["mark"], "x3 pack")
         recv = torch.empty((max(layout.total_recv, 1), ROW), dtype=torch.float32, device=dev)
         all_to_all_single(recv[:layout.total_recv], send[:layout.total_send], layout.recv_splits, layout.send_splits,
                           group)
-        _t("x4 all_to_all")
+        _t(state["mark"], "x4 all_to_all")
         vs = state["view_start"]
         N = vs[B]
         om2 = torch.empty((N, 2), dtype=torch.float32, device=dev)
@@ -334,17 +331,17 @@ class _ExchangeSplats(torch.autograd.Function):
         dev = state["flags"].device
         s = ops._stream()
         vs = state["view_start"]
-        _t("b1 loss+render backward")
+        _t(state["mark"], "b1 loss+render backward")
         g_m2, g_rgb, g_co = (None if t is None else t.contiguous() for t in (g_m2, g_rgb, g_co))
         rs, ln, cam, ds = state["segs"]
         grecv = torch.empty((max(layout.total_recv, 1), GROW), dtype=torch.float32, device=dev)
         _lib.call("gs_xchg_pack_grad", len(rs), _i32(rs), _i32(ln), _i32(cam), _i32(ds), layout.total_recv, B,
                   _row_ptrs(g_m2, vs, B), _row_ptrs(g_rgb, vs, B), _row_ptrs(g_co, vs, B), grecv.data_ptr(), s)
-        _t("b2 pack_grad")
+        _t(state["mark"], "b2 pack_grad")
         gsend = torch.empty((max(layout.total_send, 1), GROW), dtype=torch.float32, device=dev)
         all_to_all_single(gsend[:layout.total_send], grecv[:layout.total_recv], layout.send_splits, layout.recv_splits,
                           group)
-        _t("b3 all_to_all")
+        _t(state["mark"], "b3 all_to_all")
         d_m2 = torch.empty((B, P, 2), dtype=torch.float32, device=dev)
         d_rgb = torch.empty((B, P, 3), dtype=torch.float32, device=dev)
         d_co = torch.empty((B, P, 4), dtype=torch.float32, device=dev)
@@ -377,16 +374,16 @@ class _ExchangeSplatsDirect(torch.autograd.Function):
         dev = state["radii"].device
         s = ops._stream()
         N = state["view_start"][B]
-        _t("b1 loss+render backward")
+        _t(state["mark"], "b1 loss+render backward")
         _, (v_dm2, v_drgb, v_dco) = peer.views()
         for view, g in ((v_dm2, g_m2), (v_drgb, g_rgb), (v_dco, g_co)):   # into the peer-visible gradient region
             if g is None:
                 view[:N].zero_()
             else:
                 view[:N].copy_(g)
-        _t("b2 pack_grad")
+        _t(state["mark"], "b2 pack_grad")
         peer.barrier()
-        _t("b3 all_to_all")
+        _t(state["mark"], "b3 all_to_all")
         d_m2 = torch.empty((B, P, 2), dtype=torch.float32, device=dev)
         d_rgb = torch.empty((B, P, 3), dtype=torch.float32, device=dev)
         d_co = torch.empty((B, P, 4), dtype=torch.float32, device=dev)
@@ -435,8 +432,8 @@ def exchange(means2D, rgb, conic_opacity, radii, depths, strategies, settings, w
     """Per-camera view of exchange_cat (the reference's return shape, gaussian_renderer/__init__.py:1010-1023):
     a list of B tuples (means2D, rgb, conic_opacity, radii, depths) -- row slices of the concatenated tensors, empty
     where this rank renders no strip of the camera -- and the all-gathered counts."""
-    (m2, c3, co, rad, dep), view_start, cnt = exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies,
-                                                           settings, world, me, group, peer)
+    (m2, c3, co, rad, dep), view_start, cnt, _ = exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies,
+                                                              settings, world, me, group, peer)
     out = []
     for k in range(len(view_start) - 1):
         a, b = view_start[k], view_start[k + 1]
@@ -444,15 +441,18 @@ def exchange(means2D, rgb, conic_opacity, radii, depths, strategies, settings, w
     return out, cnt
 
 
-def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, settings, world, me, group=None, peer=None):
+def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, settings, world, me, group=None, peer=None,
+                 times=None, mark=None):
     """means2D (B,P,2), rgb (B,P,3), conic_opacity (B,P,4), radii (B,P) int32, depths (B,P): the local shard projected
     into the B cameras of the step (ops.preprocess_gaussians_batched, or torch.stack of per-camera results).
     peer: PeerBuffers -> splats travel by direct NVLink stores from the pack kernel into their final rows (steps where
     some rank would receive more than the regions hold, and peer=None, go through all_to_all_single).
-    Returns ((means2D (N,2), rgb (N,3), conic_opacity (N,4), radii (N), depths (N)), view_start, cnt): the splats this
-    rank has to render, all cameras concatenated in camera order (camera k = rows [view_start[k], view_start[k+1]),
-    none if the rank renders no strip of it), and the all-gathered counts cnt[i][k][j] (the reference's
-    gpui_to_gpuj_imgk_size)."""
+    times: this rank's render times for the load balancer, all-gathered behind the counts (None: no all-gather; every
+    rank must pass None alike).  mark: the diagnostics hook, called with each phase's name, in the backward too.
+    Returns ((means2D (N,2), rgb (N,3), conic_opacity (N,4), radii (N), depths (N)), view_start, cnt, gathered times): the
+    splats this rank has to render, all cameras concatenated in camera order (camera k = rows [view_start[k],
+    view_start[k+1]), none if the rank renders no strip of it), the all-gathered counts cnt[i][k][j] (the reference's
+    gpui_to_gpuj_imgk_size), and every rank's `times` as a (W, len) float32 array (None without times)."""
     B, P = means2D.shape[0], means2D.shape[1]
     # the kernels' static limits, checked HERE from values every rank shares (world, bsz, and below the all-gathered
     # counts): a rank-local failure inside a C call between two collectives would leave the other ranks hanging
@@ -479,7 +479,7 @@ def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, setting
         lo_c, hi_c = _i32(lo), _i32(hi)
         _lib.call("gs_xr_count", B, P, world, H, Wimg, _slab_ptrs(m2d, B), _slab_ptrs(radii, B), lo_c, hi_c,
                   blkcnt.data_ptr(), blkbase.data_ptr(), counts.data_ptr(), temp.data_ptr(), tb, ops._stream())
-        _t("x1 route")
+        _t(mark, "x1 route")
         # everything the pack launch needs is prepared BEFORE the all-gather is enqueued: the launch follows it closely
         rgb_c, co_c = rgb.detach().contiguous(), conic_opacity.detach().contiguous()
         pack_args = (B, P, world, H, Wimg, _slab_ptrs(m2d, B), _slab_ptrs(rgb_c, B), _slab_ptrs(co_c, B),
@@ -493,26 +493,25 @@ def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, setting
         flat =counts.t().contiguous().reshape(-1)                    # [camera k][destination j]
         allc = torch.empty((world * flat.numel(),), dtype=torch.int32, device=dev)
         dist.all_gather_into_tensor(allc, flat, group=group)          # cnt[i][k][j]
-        allp = _piggyback_gather(dev, world, group)
+        allp = _gather_times(times, dev, world, group)
         ev_counts = torch.cuda.Event()
         ev_counts.record()
         row0_dev = torch.empty((world * B + 1,), dtype=torch.int32, device=dev)
         _lib.call("gs_xr_pack_dev", *pack_args, allc.data_ptr(), me, row0_dev.data_ptr(), cap, stream)
-        _t("x3 pack")
+        _t(mark, "x3 pack")
         peer.barrier()
-        _t("x4 all_to_all")
-        global PIGGYBACK_OUT
+        _t(mark, "x4 all_to_all")
         cnt = _read_counts_on_side_stream(allc, ev_counts, (world, B, world))
-        PIGGYBACK_OUT = None if allp is None else _read_counts_on_side_stream(allp, ev_counts, (world, -1))
-        _t("x2 gather counts")
+        gathered = None if allp is None else _read_counts_on_side_stream(allp, ev_counts, (world, -1))
+        _t(mark, "x2 gather counts")
         c64 = np.asarray(cnt, dtype=np.int64)
         if peer.fits_direct(c64):   # decided from the all-gathered counts: identical on all ranks (k_xr_rows agrees)
             row0, view_start = direct_rows(c64, me)
             state = dict(group=group, radii=radii, depths=depths, m2d=m2d, blkbase=blkbase, B=B, P=P, W=world, H=H,
                          Wimg=Wimg, lo=lo_c, hi=hi_c, row0=_i32(row0), view_start=view_start, peer=peer, cnt=cnt, me=me,
-                         keep=(rgb_c, co_c))
+                         keep=(rgb_c, co_c), mark=mark)
             res = _ExchangeSplatsDirect.apply(state, means2D, rgb, conic_opacity)
-            return res, view_start, cnt
+            return res, view_start, cnt, gathered
         # does not fit the buffers this step: the row-staged path below (all_to_all_single) handles any size
         global _WARNED_OVER_CAPACITY
         if not _WARNED_OVER_CAPACITY and me == 0:
@@ -528,9 +527,9 @@ def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, setting
     temp = torch.empty((tb,), dtype=torch.uint8, device=dev)
     _lib.call("gs_xchg_route", B, P, world, H, Wimg, _slab_ptrs(m2d, B), _slab_ptrs(radii, B), _i32(lo), _i32(hi),
               flags.data_ptr(), gpos.data_ptr(), counts.data_ptr(), temp.data_ptr(), tb, ops._stream())
-    _t("x1 route")
-    cnt = gather_counts(counts.t().contiguous(), group)          # cnt[i][k][j]
-    _t("x2 gather counts")
+    _t(mark, "x1 route")
+    cnt, gathered = gather_counts(counts.t().contiguous(), group, times)   # cnt[i][k][j]
+    _t(mark, "x2 gather counts")
     nseg = int((np.asarray(cnt) > 0).sum(axis=(0, 1)).max())   # non-empty (source, camera) blocks of the busiest receiver
     if nseg >= MAX_SEGMENTS:    # identical on every rank: all raise together
         raise ValueError(f"exchange: a rank would receive {nseg} (source, camera) blocks, limit {MAX_SEGMENTS - 1}: "
@@ -540,6 +539,6 @@ def exchange_cat(means2D, rgb, conic_opacity, radii, depths, strategies, setting
     for n in layout.n_recv:
         view_start.append(view_start[-1] + n)
     state = dict(layout=layout, group=group, radii=radii, depths=depths, flags=flags, gpos=gpos, B=B, P=P, W=world,
-                 segs=segments(layout), view_start=view_start)
+                 segs=segments(layout), view_start=view_start, mark=mark)
     res = _ExchangeSplats.apply(state, means2D, rgb, conic_opacity)
-    return res, view_start, cnt
+    return res, view_start, cnt, gathered

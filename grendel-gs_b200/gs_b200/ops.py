@@ -14,7 +14,6 @@ import torch
 from . import _lib, statlog
 
 BLOCK_X, BLOCK_Y, ONE_DIM_BLOCK_SIZE = 16, 16, 256
-LAST_R_TOTAL = 0  # instances binned by the most recent render_gaussians calls (reset by the caller)
 
 
 # torch.cuda.current_stream() costs ~20 us of Python per call and every operator asks for it: a caller that runs a whole
@@ -435,8 +434,8 @@ class _RenderGaussians(torch.autograd.Function):
             pre = _instance_buffers_before_sync(key, B * T, dev, needs_grad, det)   # host work while the count / sort / scan run
             _lib.call("gs_render_count_read", ticket, C.byref(R), s)   # the operator's one host sync
             R = int(R.value)
-            global LAST_R_TOTAL
-            LAST_R_TOTAL += R
+            if collector is not None:   # the call's instance count, under the reference's name for it
+                collector["num_rendered"] = R
             ib = _instance_buffers_after_sync(key, pre, R, B * T, dev, needs_grad, det)
             seg = ib.seg if R > 0 else None
             if det:
@@ -516,7 +515,8 @@ def render_gaussians(means2D, conic_opacity, rgb, depths, radii, compute_locally
     stores every (splat, tile) instance's gradient and sums them per splat in a fixed order (gs_render_backward_det):
     two runs give the same bits.  The forward's outputs are bit-identical either way.
 
-    cuda_args: the reference's dict.  On a logging iteration (statlog.request) zhx_time "True" appends stages 24-83 of
+    cuda_args: the reference's dict.  Its stats_collector receives the call's forward / backward render times and its
+    instance count R ("num_rendered").  On a logging iteration (statlog.request) zhx_time "True" appends stages 24-83 of
     this call and b10 of its backward to the gpu_time log, and zhx_debug "True" appends this call's per-tile lines and
     summary to the n_contrib log.
 
@@ -555,7 +555,7 @@ def render_gaussians_batched(means2D, conic_opacity, rgb, depths, radii, compute
     `raster_settings` (their view / projection matrices were consumed by the preprocess).
     -> (images (B,3,H,W) with non-local tiles exactly 0, stats (B,3) int64 = n_render / n_consider / n_contrib), and
     with tile_stats=True also (B, TILE_Y, TILE_X, 3) int64: slice k is render_gaussians(..., tile_stats=True)'s for
-    camera k.  deterministic: as in render_gaussians."""
+    camera k.  cuda_args["stats_collector"] and deterministic: as in render_gaussians."""
     collector = None
     if isinstance(cuda_args, dict):
         collector = cuda_args.setdefault("stats_collector", {})

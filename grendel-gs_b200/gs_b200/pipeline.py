@@ -174,7 +174,7 @@ class Trainer:
         feedback_lag: 0 = the reference's sequencing (finish_strategy_final right after the step: the render times are
         read, all-gathered and applied before the next step starts, so the host waits for the device at the end of every
         step and cannot enqueue ahead).  > 0 (default 2, GS_B200_FEEDBACK_LAG) = the times of the step `feedback_lag`
-        steps back, whose events have long completed, ride on the NEXT exchange's size all-gather (exchange.PIGGYBACK_IN):
+        steps back, whose events have long completed, ride on the NEXT exchange's size all-gather (exchange_cat(times=...)):
         no collective of their own, no host sync; the strips move the same way, `feedback_lag` steps later.
         max_sh_degree: the SH degree the model stores (GaussianParams).
         deterministic: every render and loss of the step runs its atomic-free form (ops.render_gaussians(...,
@@ -293,7 +293,6 @@ class Trainer:
         self._bmask_cache = {}
         self._copy_stream = None
         self._loss_host = None
-        self._local_coef = None    # local sampling: (the loss weights of the local_bsz views, the constant term)
         self._info = {}
         self._h2d = 0
 
@@ -384,11 +383,11 @@ class Trainer:
         order (a camera may appear more than once); None = all cameras in order.  The caller chooses them (the reference
         draws --bsz per step, train_internal.py:134).  resident=False copies the GT strips from pinned host memory inside
         the step and reads the loss back (the end-to-end leg); returns the loss as a float then.
-        With local_sampling, views are this rank's own local_bsz views (required), and the step is _step_local."""
+        With local_sampling, views are this rank's own local_bsz views (required)."""
         views = self._local_views(views) if self.local_sampling else self._batch_views(views)
         ops.STEP_STREAM = torch.cuda.current_stream().cuda_stream   # every kernel of the step goes to this stream
         try:
-            return self._step_local(views, resident) if self.local_sampling else self._step(views, resident)
+            return self._step(views, resident)
         finally:
             ops.STEP_STREAM = None
 
@@ -484,16 +483,16 @@ class Trainer:
 
     @contextlib.contextmanager
     def _eval_state(self):
-        """Forward-only scoring: no gradients, no tracing, every kernel on the current stream; the step's globals are
-        restored afterwards."""
-        saved = (ops.LAST_R_TOTAL, getattr(self, "_trace_on", False), self._ex.TRACE, ops.STEP_STREAM)
-        self._trace_on, self._ex.TRACE = False, None
+        """Forward-only scoring: no gradients, no tracing, every kernel on the current stream; the tracing switch and the
+        operators' pinned stream are restored afterwards."""
+        saved = (getattr(self, "_trace_on", False), ops.STEP_STREAM)
+        self._trace_on = False
         ops.STEP_STREAM = torch.cuda.current_stream().cuda_stream
         try:
             with torch.no_grad():
                 yield
         finally:
-            ops.LAST_R_TOTAL, self._trace_on, self._ex.TRACE, ops.STEP_STREAM = saved
+            self._trace_on, ops.STEP_STREAM = saved
 
     def _eval_batches(self, dcams, host, views, bsz, held_out):
         """The batches of an evaluation, bsz views each: a fresh strip division of the listed views (one history per
@@ -527,8 +526,8 @@ class Trainer:
                     gts.append(host[bviews[k]]); gt_row0.append(0)
                 else:
                     gts.append(self._strip_h2d(host[bviews[k]], r[0], r[1])); gt_row0.append(r[0])
-            collectors = [{} for _ in bcams]
-            fw = self._forward(settings, strategies, collectors, lambda: ops.pack_cameras(settings), training=False)
+            fw = self._forward(settings[0], strategies, {}, lambda: ops.pack_cameras(settings), (0, len(bcams)),
+                               training=False)
             yield strategies, rows, gts, gt_row0, fw
 
     def _sum_slots_over_ranks(self, slots):
@@ -628,60 +627,6 @@ class Trainer:
         self._batch_table = torch.index_select(self._cam_table_dev, 0, idx)
         return self._batch_table
 
-    def _step_local(self, views, resident):
-        """One local-sampling step.  Every rank projects its Gaussian shard into all B = W x local_bsz views of the batch
-        (the camera table gathered on the device), the exchange hands each rank the splats of its own views, and the rank
-        renders them whole in one batched render and scores them against its own images.  No timing feedback: the
-        division does not read it."""
-        self._trace_on = False
-        self._ex.TRACE = None
-        p = self.params
-        for t in p.raw_parameters():
-            t.grad = None
-        self._h2d = 0
-        ops.LAST_R_TOTAL = 0
-        k, B, H = self.local_bsz, self.world * self.local_bsz, self.H
-        strategies = self._whole_view_division()
-        rs = self.dcams[views[0]].settings(p.active_sh_degree)   # image size and background, shared by every view
-        # the whole own images from pinned host memory, on the copy stream, while the render runs
-        gt_ready = [] if resident else [self._copy_gt(v, 0, H) for v in views]
-        batched = self._preprocess(rs, lambda: self._gathered_camera_table(views), B, training=True)
-        self.means2D, self._radii_local = batched[0], batched[3]
-        if self.world > 1:
-            self._ex.PIGGYBACK_IN = None   # no render times ride on the exchange
-            cat, view_start, _cnt = self._ex.exchange_cat(*batched, strategies, [rs], self.world, self.rank, self.group,
-                                                          self._peer)
-            view_start = view_start[self.rank * k:(self.rank + 1) * k + 1]   # the other views have no rows here
-        else:
-            cat, view_start = self._concat(batched)
-        collectors = [{} for _ in range(k)]
-        m2, rgb, co, radii, depths = cat
-        images, _stats = ops.render_gaussians_batched(m2, co, rgb, depths, radii, None, view_start, rs,
-                                                      {"stats_collector": collectors[0]}, deterministic=self.deterministic)
-        # the whole resident images, read in place, or the copies once they have landed
-        gts = [self.gts_dev[v] for v in views] if resident else [self._wait_gt(r) for r in gt_ready]
-        if self._local_coef is None:   # the weights and constant the default batched step forms for whole strips
-            coef, const = [], 0.0
-            for _ in range(k):
-                coef += [1.0 - self.lambda_dssim, -self.lambda_dssim]
-                const += self.lambda_dssim
-            self._local_coef = (torch.tensor(coef, dtype=torch.float32, device=self.device), const)
-        coef, const = self._local_coef
-        l1_ssim = ops.fused_l1_ssim_batched(images, gts, [(0, H, 0, H)] * k, deterministic=self.deterministic,
-                                            gt_full=resident)
-        loss_sum = torch.dot(l1_ssim.reshape(-1), coef) + const
-        loss_sum.backward()
-        self._finish_local_step(strategies, collectors, int(view_start[-1]) - int(view_start[0]))
-        if resident:
-            return None
-        return self._read_loss(loss_sum)
-
-    def _finish_local_step(self, strategies, collectors, n_splats):
-        """The host bookkeeping after a local-sampling step.  Nothing is queued for the load balancer."""
-        self._collectors, self._strategies = collectors, strategies
-        self._counts = dict(Vp=n_splats, P_local=self.local_bsz * self.H * self.W)
-        self.iteration += 1
-
     def _read_loss(self, loss_sum):
         """The step's loss as a float, through a pinned host word (the resident=False leg)."""
         if self._loss_host is None:
@@ -730,10 +675,20 @@ class Trainer:
             self._cams_dev = (views, stage.to(self.device, non_blocking=True))
         return self._cams_dev[1]
 
+    def _step_plan(self, views):
+        """What sets a local-sampling step apart from the default one, decided once at the top of the step.
+        -> (the batch's division, cam_table() -> its (B,40) device camera table, the span (lo, hi) of the batch positions
+        this rank renders -- position p is the view views[p - lo] --, whether the render times are fed back)."""
+        if self.local_sampling:   # the B = W x local_bsz views of all ranks, each rendered whole by the rank that drew it
+            k = self.local_bsz
+            return (self._whole_view_division(), lambda: self._gathered_camera_table(views),
+                    (self.rank * k, (self.rank + 1) * k), False)
+        strategies = self._batch_strategies(tuple(self.dcams[i].uid for i in views))
+        return strategies, lambda: self._camera_table(views), (0, len(views)), True
+
     def _step(self, views, resident):
         import os as _os, time as _time
         self._trace_on = _os.environ.get("GS_B200_TRACE") == "1"
-        self._ex.TRACE = self._mark if self._trace_on else None
         if self._trace_on:
             if not hasattr(self, "trace"):
                 self.trace = {}
@@ -743,32 +698,30 @@ class Trainer:
         for t in p.raw_parameters():
             t.grad = None
         self._h2d = 0
-        ops.LAST_R_TOTAL = 0
-        dcams = [self.dcams[i] for i in views]
-        strategies = self._batch_strategies(tuple(c.uid for c in dcams))
-        self._tasks = [[(k, st.division_pos[st.gpu_ids.index(g)], st.division_pos[st.gpu_ids.index(g) + 1])
-                        for k, st in enumerate(strategies) if g in st.gpu_ids] for g in range(self.world)]
-        settings = [c.settings(p.active_sh_degree) for c in dcams]
+        strategies, cam_table, (lo, hi), feedback = self._step_plan(views)
+        rs = self.dcams[views[0]].settings(p.active_sh_degree)   # image size and background, shared by every view
         # "Asynchronously load ground-truth image to GPU" (loss_distribution.py:2399): the strips this rank needs are
         # copied from pinned host memory on a side stream while preprocess / binning / blend run, and the loss waits
         # on the copy's event.
         gt_ready = {}
         if not resident and self.distributed_dataset_storage:
             from . import gt_scatter
+            tasks = [[(k, st.division_pos[st.gpu_ids.index(g)], st.division_pos[st.gpu_ids.index(g) + 1])
+                      for k, st in enumerate(strategies) if g in st.gpu_ids] for g in range(self.world)]
             batch_host = [self.gts_host[i] for i in views] if self.rank == 0 else self.W
-            strips, h2d = gt_scatter.scatter_gt_strips(batch_host, self._tasks, self.H,
-                                                       self.device, self.rank, self.world, self.group)
+            strips, h2d = gt_scatter.scatter_gt_strips(batch_host, tasks, self.H, self.device, self.rank, self.world,
+                                                       self.group)
             self._h2d += h2d
             ev = torch.cuda.Event()
             ev.record(torch.cuda.current_stream())
             gt_ready = {k: (t, ev) for k, t in strips.items()}
         elif not resident:
-            for k, st in enumerate(strategies):
+            for k, st in enumerate(strategies[lo:hi]):
                 rows = st.local_pixel_rows(self.H)
                 if rows is not None:
                     gt_ready[k] = self._copy_gt(views[k], rows[0], rows[1])
-        collectors = [{} for _ in dcams]
-        fw = self._forward(settings, strategies, collectors, lambda: self._camera_table(views), training=True)
+        collectors = [{} for _ in range(hi - lo)]
+        fw = self._forward(rs, strategies, collectors[0], cam_table, (lo, hi), training=True, feedback=feedback)
         self.means2D, self._radii_local = fw.means2D, fw.radii
         if self.border_exchange:
             # the legacy row L1: one loss per local strip, summed in view order; a strip of a view split over several
@@ -801,14 +754,20 @@ class Trainer:
         self._mark("r render+loss")
         loss_sum.backward()
         self._mark("b4 backward (rest)")
-        self._collectors, self._strategies = collectors, strategies
-        self._counts = dict(Vp=int(fw.view_start[-1]), P_local=sum((r[1] - r[0]) * self.W for r in fw.rows4))
-        self.iteration += 1
-        self._feed_back_times(strategies, collectors)
+        self._finish_step(strategies, collectors, dict(Vp=int(fw.view_start[-1]) - int(fw.view_start[0]),
+                                                       P_local=sum((r[1] - r[0]) * self.W for r in fw.rows4)), feedback)
         self._mark("t time feedback")
         if resident:
             return None
         return self._read_loss(loss_sum)
+
+    def _finish_step(self, strategies, collectors, counts, feedback):
+        """The host bookkeeping after a step, and with feedback its render times queued for (or, with feedback_lag=0,
+        applied to) the load balancer."""
+        self._collectors, self._strategies, self._counts = collectors, strategies, counts
+        self.iteration += 1
+        if feedback:
+            self._feed_back_times(strategies, collectors)
 
     def _copy_gt(self, view, y0, y1):
         """Rows [y0, y1) of a view's host image, copied on the side stream while preprocess / binning / blend run.
@@ -853,33 +812,33 @@ class Trainer:
         B, Pn = batched[0].shape[:2]
         return tuple(t.reshape(B * Pn, *t.shape[2:]) for t in batched), [k * Pn for k in range(B + 1)]
 
-    def _forward(self, settings, strategies, collectors, cam_table, training):
+    def _forward(self, rs, strategies, collector, cam_table, span, training, feedback=False):
         """The forward of one batch: preprocess (_preprocess) -> exchange of the projected splats (exchange_cat, W > 1) or
-        their concatenation (W == 1) -> one batched render of every local strip.  cam_table(): the (B,40) device camera
-        table of the batched preprocess.  training=False (evaluate): no screen-space gradient is retained and no render
-        times ride on the exchange.
+        their concatenation (W == 1) -> one batched render of the batch positions span = (lo, hi): every position for the
+        strip division, this rank's own views for local sampling.  rs: the raster settings the views share (a one-view
+        batch's own).  cam_table(): the (B,40) device camera table of the batched preprocess.  collector: the render's
+        stats collector.  training: the screen-space gradient is retained (evaluate: not).  feedback: the load balancer's
+        render times ride on the exchange.
         -> namespace of means2D (B,P,2) and radii (B,P) (this rank's pre-exchange values, which densification reads),
-        images (B,3,H,W), the local strips' rows4 and loss weights coef / const, and view_start."""
-        B = len(settings)
-        batched = self._preprocess(settings[0], cam_table, B, training)
+        images (hi - lo,3,H,W), the span's rows4 and loss weights coef / const, and its view_start."""
+        B, (lo, hi) = len(strategies), span
+        batched = self._preprocess(rs, cam_table, B, training)
         self._mark("p preprocess")
         if self.world > 1:
-            if training:
-                self._feedback_before_exchange()
-            else:
-                self._ex.PIGGYBACK_IN = None
-            cat, view_start, _cnt = self._ex.exchange_cat(*batched, strategies, settings, self.world, self.rank,
-                                                          self.group, self._peer)
-            if training:
-                self._feedback_after_exchange()
+            times = self._feedback_before_exchange() if feedback else None
+            cat, view_start, _cnt, gathered = self._ex.exchange_cat(*batched, strategies, [rs], self.world, self.rank,
+                                                                    self.group, self._peer, times=times, mark=self._mark)
+            if feedback:
+                self._feedback_after_exchange(gathered)
         else:
             cat, view_start = self._concat(batched)
         self._mark("x5 unpack")
-        mk = tuple((tuple(st.gpu_ids), tuple(st.division_pos), st.rank) for st in strategies)
+        view_start = view_start[lo:hi + 1]   # the positions outside the span have no rows here
+        mk = (span, tuple((tuple(st.gpu_ids), tuple(st.division_pos), st.rank) for st in strategies))
         if mk not in self._bmask_cache:
-            m = torch.zeros((B, self.tile_y, self.tile_x), dtype=torch.uint8, device=self.device)
+            m = torch.zeros((hi - lo, self.tile_y, self.tile_x), dtype=torch.uint8, device=self.device)
             rows4, coef, const = [], [], 0.0
-            for k, st in enumerate(strategies):
+            for k, st in enumerate(strategies[lo:hi]):
                 r = st.local_rows()
                 if r is None:   # no strip of this camera here: no tiles, no loss term
                     rows4.append((0, 0, 0, 0))
@@ -890,12 +849,12 @@ class Trainer:
                 rows4.append((y0, y1, y0, y1))
                 coef += [1.0 - self.lambda_dssim, -self.lambda_dssim]
                 const += self.lambda_dssim
-            self._bmask_cache[mk] = (m.reshape(B, -1), rows4,
+            self._bmask_cache[mk] = (m.reshape(hi - lo, -1), rows4,
                                      torch.tensor(coef, dtype=torch.float32, device=self.device), const)
         cl, rows4, coef, const = self._bmask_cache[mk]
         m2, rgb, co, radii, depths = cat
-        images, _stats = ops.render_gaussians_batched(m2, co, rgb, depths, radii, cl, view_start, settings[0],
-                                                      {"stats_collector": collectors[0]}, deterministic=self.deterministic)
+        images, _stats = ops.render_gaussians_batched(m2, co, rgb, depths, radii, cl, view_start, rs,
+                                                      {"stats_collector": collector}, deterministic=self.deterministic)
         return SimpleNamespace(means2D=batched[0], radii=batched[3], images=images, rows4=rows4, coef=coef, const=const,
                                view_start=view_start)
 
@@ -915,20 +874,21 @@ class Trainer:
         return mine
 
     def _feedback_before_exchange(self):
-        """feedback_lag > 0: hand the render times of the step `feedback_lag` steps back (its events have completed: the
-        host is never more than one step ahead of the device) to the exchange, which all-gathers them behind the sizes."""
-        self._ex.PIGGYBACK_IN, self._sent_feedback = None, None
+        """feedback_lag > 0: the render times of the step `feedback_lag` steps back (its events have completed: the host is
+        never more than one step ahead of the device), for the exchange to all-gather behind the sizes -> this rank's
+        times, or None when no step's feedback is due."""
+        self._sent_feedback = None
         if self.feedback_lag > 0 and len(self._pending_feedback) >= self.feedback_lag:
-            entry = self._pending_feedback.pop(0)
-            self._ex.PIGGYBACK_IN = self._times_of(entry[0], entry[1])
-            self._sent_feedback = entry
+            self._sent_feedback = self._pending_feedback.pop(0)
+            return self._times_of(self._sent_feedback[0], self._sent_feedback[1])
+        return None
 
-    def _feedback_after_exchange(self):
+    def _feedback_after_exchange(self, times):
+        """times: every rank's times as the exchange all-gathered them, (W, B) (None: none were sent)."""
         if self._sent_feedback is None:
             return
         strategies, _collectors, iteration = self._sent_feedback
-        times = self._ex.PIGGYBACK_OUT
-        self._ex.PIGGYBACK_IN, self._sent_feedback = None, None
+        self._sent_feedback = None
         if times is not None:
             finish_strategy(self.history, strategies, times.tolist(), iteration, self.world, self.H, self.W,
                             self.heuristic_decay)
@@ -980,7 +940,7 @@ class Trainer:
     def last_info(self):
         """Realised sizes of the last step on this rank: V visible, V' splats rendered, R instances."""
         V = int((self._radii_local > 0).sum())
-        R = ops.LAST_R_TOTAL
+        R = self._collectors[0]["num_rendered"]   # the step's one render
         return dict(V=V, Vp=self._counts["Vp"], P_local=self._counts["P_local"], R=R)
 
     def io_bytes_per_step(self):

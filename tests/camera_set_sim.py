@@ -7,7 +7,7 @@ process group) and then told their rank and world size."""
 import numpy as np
 import torch
 
-from gs_b200 import division, exchange, pipeline
+from gs_b200 import division, pipeline
 from gs_b200 import synthetic as syn
 
 
@@ -29,15 +29,11 @@ class SimRanks:
         uids = tuple(self.trs[0].dcams[i].uid for i in views)
         strategies = [tr._batch_strategies(uids) for tr in self.trs]
         # the exchange: every rank hands its piggybacked times in, the all-gather hands all of them out
-        ins = []
-        for tr in self.trs:
-            tr._feedback_before_exchange()
-            ins.append(exchange.PIGGYBACK_IN)
+        ins = [tr._feedback_before_exchange() for tr in self.trs]
         assert all((x is None) == (ins[0] is None) for x in ins)
+        gathered = None if ins[0] is None else np.asarray(ins, dtype=np.float32)
         for tr in self.trs:
-            exchange.PIGGYBACK_OUT = None if ins[0] is None else np.asarray(ins, dtype=np.float32)
-            tr._feedback_after_exchange()
-        exchange.PIGGYBACK_IN = exchange.PIGGYBACK_OUT = None
+            tr._feedback_after_exchange(gathered)
         times = []
         for r, (tr, sts) in enumerate(zip(self.trs, strategies)):
             # one batched render per rank: its time is the sum over the rank's strips, in collectors[0]

@@ -99,8 +99,8 @@ def views_check(dev, rank, world, B, scene, log, oracle):
         outs = []
         for peer in (tr._peer, None):
             leaves = [stacked[q].detach().clone().requires_grad_(True) for q in range(3)]
-            (m2, c3, co, rad, dep), vs, _ = tr._ex.exchange_cat(leaves[0], leaves[1], leaves[2], stacked[3], stacked[4],
-                                                                strategies, settings, world, rank, None, peer)
+            (m2, c3, co, rad, dep), vs, _, _ = tr._ex.exchange_cat(leaves[0], leaves[1], leaves[2], stacked[3], stacked[4],
+                                                                   strategies, settings, world, rank, None, peer)
             gen = torch.Generator(device=dev).manual_seed(7 + rank)
             up = [torch.randn(t.shape, device=dev, generator=gen) for t in (m2, c3, co)]
             ((m2 * up[0]).sum() + (c3 * up[1]).sum() + (co * up[2]).sum()).backward()

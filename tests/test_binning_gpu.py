@@ -327,16 +327,16 @@ def sequence_scenes(W=1920, H=1080):
     return out
 
 
-def op_render(c, batched, grad, g_seed=0):
+def op_render(c, batched, grad, g_seed=0, cuda_args=None):
     from gs_b200 import ops
     W, H = c["W"], c["H"]
     m2, co, rgb, d, rad = op_inputs(c, grad)
     rs = settings(W, H)
     if batched:
         P = len(c["radii"])
-        img, _ = ops.render_gaussians_batched(m2, co, rgb, d, rad, None, [0, P // 3, P], rs)
+        img, _ = ops.render_gaussians_batched(m2, co, rgb, d, rad, None, [0, P // 3, P], rs, cuda_args)
     else:
-        img, *_ = ops.render_gaussians(m2, co, rgb, d, rad, None, rs)
+        img, *_ = ops.render_gaussians(m2, co, rgb, d, rad, None, rs, cuda_args)
     return img, (m2, co, rgb)
 
 
@@ -348,7 +348,7 @@ def backward(img, leaves, seed=0):
 
 @pytest.mark.parametrize("batched", [False, True], ids=["single", "batched"])
 @pytest.mark.parametrize("grad", [False, True], ids=["forward", "grad"])
-def test_instance_hints_across_jumping_R(batched, grad):
+def test_instance_hints_and_counts_across_jumping_R(batched, grad):
     from gs_b200 import ops
     scenes = sequence_scenes()
     alone = []
@@ -359,9 +359,9 @@ def test_instance_hints_across_jumping_R(batched, grad):
     ops._R_HINT.clear()
     Rs = []
     for c, (img0, g0) in zip(scenes, alone):
-        before = ops.LAST_R_TOTAL
-        img, leaves = op_render(c, batched, grad)
-        Rs.append(ops.LAST_R_TOTAL - before)
+        collector = {}
+        img, leaves = op_render(c, batched, grad, cuda_args={"stats_collector": collector})
+        Rs.append(collector["num_rendered"])
         assert torch.equal(img.detach(), img0)
         if grad:
             for a, b, name in zip(backward(img, leaves), g0, ("means2D", "conic_opacity", "rgb")):

@@ -67,7 +67,7 @@ def test_strategy_cache_is_keyed_by_uids():
 
 
 @pytest.mark.parametrize("lag", [2, 1])
-def test_feedback_updates_the_cameras_it_was_measured_on(lag):
+def test_feedback_passed_by_value_updates_the_cameras_it_was_measured_on(lag):
     """Each camera's cost heuristic -- and so its division -- changes only from the times measured on the steps it was
     in, applied `lag` steps later, also when it is absent from the batch the feedback arrives with."""
     cams = cams_of(6, BIG_W, BIG_H)

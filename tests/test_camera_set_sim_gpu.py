@@ -14,7 +14,7 @@ DEV = torch.device("cuda", 0)
 BIG_W, BIG_H = 1936, 1088   # large enough that the reference re-estimates row costs for every batch size
 
 
-def test_each_camera_moves_only_from_its_own_render_times():
+def test_each_camera_moves_only_from_its_own_gathered_render_times():
     cams = [syn.make_camera(BIG_W, BIG_H, yaw_deg=12.0 * k - 30.0, uid=7 + k) for k in range(6)]
     uid_to_cam = {c["uid"]: k for k, c in enumerate(cams)}
     params = pipeline.GaussianParams(syn.make_scene(200_000, BIG_W, BIG_H, seed=4), DEV)

@@ -159,14 +159,12 @@ def _worker(rank, world, port, B, P, tile_y, q):
         local_counts = torch.zeros((B, world), dtype=torch.int32)
         for k in range(B):
             local_counts[k, torch.tensor(gpu_ids[k])] = masks[k].sum(0).to(torch.int32)
-        # the timing feedback rides on the size all-gather (exchange.PIGGYBACK_IN / _OUT): every rank gets every rank's row
-        exchange.PIGGYBACK_IN = [rank + 0.5] + [-1.0] * (B - 1)
-        cnt = exchange.gather_counts(local_counts)
-        fb = exchange.PIGGYBACK_OUT
-        exchange.PIGGYBACK_IN = None
+        # the timing feedback rides on the size all-gather (gather_counts(times=...)): every rank gets every rank's row
+        cnt, fb = exchange.gather_counts(local_counts, times=[rank + 0.5] + [-1.0] * (B - 1))
         assert fb is not None and fb.shape == (world, B)
         assert fb[:, 0].tolist() == [r + 0.5 for r in range(world)] and (fb[:, 1:] == -1.0).all()
-        assert exchange.gather_counts(local_counts).tolist() == cnt.tolist() and exchange.PIGGYBACK_OUT is None
+        cnt_again, fb = exchange.gather_counts(local_counts)
+        assert cnt_again.tolist() == cnt.tolist() and fb is None
         lay = exchange.Layout(cnt, rank, gpu_ids)
         # torch emulation of gs_pack_rows
         send = torch.full((lay.total_send, exchange.ROW), -1.0)
@@ -219,7 +217,7 @@ def _worker(rank, world, port, B, P, tile_y, q):
 
 
 @pytest.mark.parametrize("world,B,tile_y", [(2, 1, 68), (2, 2, 25), (3, 4, 40)])
-def test_exchange_layout_over_gloo(world, B, tile_y):
+def test_exchange_layout_and_gathered_times_over_gloo(world, B, tile_y):
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = _free_port()

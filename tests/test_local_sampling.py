@@ -219,7 +219,7 @@ def no_load_balancer(monkeypatch):
 
 
 @pytest.mark.parametrize("world,k", [(2, 2), (4, 1), (3, 3)])
-def test_simulated_ranks_never_touch_the_history(no_load_balancer, world, k):
+def test_simulated_ranks_never_touch_the_history_or_send_feedback(no_load_balancer, world, k):
     n = 12
     cams = cams_of(n)
     trs = []
@@ -236,8 +236,9 @@ def test_simulated_ranks_never_touch_the_history(no_load_balancer, world, k):
         union = torch.tensor([v for m in mine for v in m], dtype=torch.int64)   # the all-gather, in rank order
         for r, tr in enumerate(trs):
             assert tr._local_views(list(mine[r])) == mine[r]
-            sts = tr._whole_view_division()
+            sts, _cam_table, span, feedback = tr._step_plan(mine[r])
             assert sts is tr._whole_view_division()                      # built once
+            assert span == (r * k, (r + 1) * k) and not feedback          # its own positions, no timing feedback
             # each position is rendered whole by the rank that sampled it and holds its image
             for p, st in enumerate(sts):
                 owner = p // k
@@ -245,8 +246,8 @@ def test_simulated_ranks_never_touch_the_history(no_load_balancer, world, k):
                 assert tr.gts_host[int(union[p])] is not None if owner == r else True
             table = torch.index_select(tr._cam_table_dev, 0, union)       # the device-side gather, on the CPU
             assert torch.equal(table, full[union]) and torch.equal(table, tr._cam_rows[union])
-            tr._finish_local_step(sts, [{} for _ in range(k)], 0)
-        assert exchange.PIGGYBACK_IN is None
+            tr._finish_step(sts, [{} for _ in range(k)], dict(Vp=0, P_local=k * TH * TW), feedback)
+            assert tr._sent_feedback is None and tr._pending_feedback == []
     for tr in trs:
         assert tr.iteration == 6
         assert tr.history.history == [] and tr.balance_log == [] and tr._pending_feedback == []

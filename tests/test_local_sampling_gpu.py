@@ -62,14 +62,14 @@ def assert_same_step(a, b, what):
 
 def assert_no_load_balancer(tr):
     assert tr.history.history == [] and tr.balance_log == [] and tr._pending_feedback == []
-    assert tr._strategy_cache is None and exchange.PIGGYBACK_IN is None
+    assert tr._strategy_cache is None and tr._sent_feedback is None
     assert all(torch.equal(h, torch.ones(tr.tile_y)) for h in tr.history.accum_heuristic.values())
 
 
 # (a) one rank: the local-sampling step is the default step
 @pytest.mark.parametrize("views", [[7, 2, 9, 0], [5], [3, 3]])
 @pytest.mark.parametrize("resident", [True, False])
-def test_one_rank_equals_the_default_trainer(camera_set, views, resident):
+def test_one_rank_local_step_is_the_default_step(camera_set, views, resident):
     scene, cams, gts = camera_set
     default, local = pair(scene, cams, gts, len(views))
     la = default.step(views=views, resident=resident)
@@ -105,7 +105,7 @@ def _densify(opt, accum, denom, params, noise):
 
 
 @pytest.mark.parametrize("k", [4, 1])
-def test_one_rank_training_run_equals_the_default_trainer(camera_set, k):
+def test_one_rank_local_training_run_is_the_default_run(camera_set, k):
     """Six steps over changing views with FusedAdam and a densify/prune after the third: the same losses, gradients,
     statistics, densification counts and parameters, bit for bit."""
     scene, cams, gts = camera_set
