@@ -113,6 +113,8 @@ SIGNATURES = {
     "gs_xchg_scatter_grad": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gs_adam_step": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_float, _vp]),
     "gs_knn3_mean_dist2": (_i, [_i, _vp, _vp, _vp]),
+    "gs_knn3_temp_bytes": (_sz, [_i]),
+    "gs_knn3_mean_dist2_range": (_i, [_i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
     "gs_densify_temp_bytes": (_sz, [_i]),
     "gs_densify_select": (_i, [_i, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _real, _real, _i, _vp, _sz, _vp, _vp]),
     "gs_densify_gather": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -121,11 +121,19 @@ class PlyLayout(NamedTuple):
     max_sh_degree: int
 
 
-def read_ply_header(path, max_sh_degree=None):
-    """Parse and check a PLY header.  Accepts comment / obj_info lines, any property order and extra scalar properties;
-    refuses, with a ValueError naming the file: ascii or big-endian data, a first element other than `vertex`, list
-    properties, a needed attribute that is missing or not float, an f_rest count other than 3K - 3 for the requested
-    degree (any degree 0..3 when max_sh_degree is None) and a body shorter than the vertex records."""
+class PlyVertices(NamedTuple):
+    """The vertex element of a checked binary little-endian PLY file."""
+    n: int                   # vertices
+    types: dict              # property name -> PLY type name
+    dtype: np.dtype          # one vertex record
+    body: int                # byte offset of the first vertex
+
+
+def parse_ply_vertices(path):
+    """Parse the generic part of a PLY header.  Accepts comment / obj_info lines, any property order and extra scalar
+    properties; refuses, with a ValueError naming the file: ascii or big-endian data, a first element other than
+    `vertex`, list properties in it and unknown or repeated properties.  A reader checks the properties it needs, then
+    the body's length (check_ply_body), so a file with several faults is named for the same one whichever reader."""
     with open(path, "rb") as f:
         head = f.read(1 << 16)
         while b"end_header\n" not in head:
@@ -170,7 +178,33 @@ def read_ply_header(path, max_sh_degree=None):
     types = dict(props)
     if len(types) != len(props):
         raise ValueError(f"{path}: a vertex property name appears twice")
-    n_rest = sum(1 for name, _ in props if re.fullmatch(r"f_rest_\d+", name))
+    return PlyVertices(n, types, np.dtype([(name, _PLY_TYPES[t]) for name, t in props]), end)
+
+
+def check_ply_body(path, vertices):
+    """Refuses, with a ValueError naming the file, a body shorter than the vertex records of parse_ply_vertices."""
+    n, _, dtype, end = vertices
+    if os.path.getsize(path) < end + n * dtype.itemsize:
+        raise ValueError(f"{path}: truncated: {n} vertices of {dtype.itemsize} bytes need "
+                         f"{end + n * dtype.itemsize} bytes, the file has {os.path.getsize(path)}")
+
+
+def read_ply_vertices(path, dtype, body, a, b):
+    """Vertex records [a, b) of a checked file (parse_ply_vertices' dtype and body) -> numpy structured array."""
+    with open(path, "rb") as f:
+        f.seek(body + a * dtype.itemsize)
+        buf = bytearray((b - a) * dtype.itemsize)   # writable: torch.from_numpy takes it without a copy
+        f.readinto(buf)
+    return np.frombuffer(buf, dtype=dtype, count=b - a)
+
+
+def read_ply_header(path, max_sh_degree=None):
+    """Parse and check a PLY header of a model: parse_ply_vertices, then refuses, with a ValueError naming the file, a
+    needed attribute that is missing or not float and an f_rest count other than 3K - 3 for the requested degree (any
+    degree 0..3 when max_sh_degree is None), then check_ply_body."""
+    vertices = parse_ply_vertices(path)
+    n, types, dtype, end = vertices
+    n_rest = sum(1 for name in types if re.fullmatch(r"f_rest_\d+", name))
     if max_sh_degree is None:
         if n_rest not in (0, 9, 24, 45):
             raise ValueError(f"{path}: {n_rest} f_rest properties is no SH degree 0..3 (0, 9, 24 or 45)")
@@ -185,10 +219,7 @@ def read_ply_header(path, max_sh_degree=None):
             raise ValueError(f"{path}: attribute {a!r} is missing")
         if _PLY_TYPES[types[a]] != "<f4":
             raise ValueError(f"{path}: attribute {a!r} is {types[a]}, not float")
-    dtype = np.dtype([(name, _PLY_TYPES[t]) for name, t in props])
-    if os.path.getsize(path) < end + n * dtype.itemsize:
-        raise ValueError(f"{path}: truncated: {n} vertices of {dtype.itemsize} bytes need "
-                         f"{end + n * dtype.itemsize} bytes, the file has {os.path.getsize(path)}")
+    check_ply_body(path, vertices)
     return PlyLayout(path, n, dtype, end, int(max_sh_degree))
 
 
@@ -196,11 +227,7 @@ def read_ply_rows(layout, a=0, b=None):
     """Vertices [a, b) of a checked file -> (b - a, F) float32 rows in attribute_names order (normals zero)."""
     b = layout.n if b is None else b
     names = attribute_names(layout.max_sh_degree)
-    with open(layout.path, "rb") as f:
-        f.seek(layout.body + a * layout.dtype.itemsize)
-        buf = bytearray((b - a) * layout.dtype.itemsize)   # writable: torch.from_numpy takes it without a copy
-        f.readinto(buf)
-    rec = np.frombuffer(buf, dtype=layout.dtype, count=b - a)
+    rec = read_ply_vertices(layout.path, layout.dtype, layout.body, a, b)
     if list(layout.dtype.names) == names:   # the layout this module writes: the records are the rows
         return rec.view("<f4").reshape(b - a, len(names))
     rows = np.zeros((b - a, len(names)), dtype="<f4")

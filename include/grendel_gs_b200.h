@@ -652,9 +652,19 @@ GS_API int gs_densify_stats(int num_views, int P, const void *const *grad_host, 
 
 /* ---- simple_knn._C.distCUDA2 -- /root/reference/scene/gaussian_model.py:20,163-166 ------------------------------------
  * Mean squared distance of every point to its 3 nearest OTHER points (self excluded by index, duplicates count at
- * distance 0; fewer than 3 other points: the mean of those that exist), the start-up scale initialisation.  Exact, by
- * tiled brute force (init-time only).  points (N,3) fp32 -> mean_dist2 (N) fp32.  NOT yet run on a device. */
+ * distance 0; fewer than 3 other points: the mean of those that exist), the start-up scale initialisation.
+ * gs_knn3_mean_dist2: the exhaustive tiled brute force, O(N^2), kept as the reference the search is tested against.
+ * points (N,3) fp32 -> mean_dist2 (N) fp32. */
 GS_API int gs_knn3_mean_dist2(int N, const float *points, float *mean_dist2, void *stream);
+/* gs_knn3_mean_dist2_range: the same values, bit for bit, for the queries [q0, q1) against all N points, by an exact
+ * Morton-tree search (DESIGN.md 5i): out (q1 - q0) fp32, out[i - q0] for point i.  points and out 4-byte aligned, temp
+ * 16-byte aligned and at least gs_knn3_temp_bytes(N) bytes (GS_ENOMEM otherwise).  The size depends on the current
+ * device (CUB's scratch): where no device can be queried, gs_knn3_temp_bytes returns 0 and the search GS_ECUDA, after
+ * the argument checks.  Reads the cloud's bounding box back once (synchronises `stream`) and refuses a non-finite
+ * coordinate with GS_EINVAL before the search.  q0 == q1: no work, pointers not read. */
+GS_API size_t gs_knn3_temp_bytes(int N);
+GS_API int gs_knn3_mean_dist2_range(int N, const float *points, int q0, int q1, float *out, void *temp,
+                                    size_t temp_bytes, void *stream);
 
 /* ---- legacy tile-mask / tile-exchange helpers (SURVEY.md 8a rows L3-L4; dead code in the shipped trainer) ------
  * _C.get_touched_locally                     -- gaussian_renderer/loss_distribution.py:136-141
