@@ -791,8 +791,9 @@ class Trainer:
 
     def _preprocess(self, rs, cam_table, B, training):
         """This rank's Gaussians projected into the B views of a batch -> (means2D (B,P,2), rgb, conic_opacity, radii,
-        depths).  One view runs the per-camera kernel with its settings rs; more run ONE batched launch over the (B,40)
-        device camera table cam_table(), which reads every Gaussian once.  training: means2D keeps its gradient, which
+        depths).  One view runs the per-camera kernel with its settings rs, whose backward is faster than the batched
+        one's at B = 1 (DESIGN.md section 5); more run ONE batched launch over the (B,40) device camera table
+        cam_table(), which reads every Gaussian once.  training: means2D keeps its gradient, which
         densification reads (means2D.grad of camera k, densification.py:24)."""
         p = self.params
         if B == 1:
