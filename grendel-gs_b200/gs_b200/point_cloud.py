@@ -103,5 +103,14 @@ def cameras_extent(cams):
     if not len(cams):
         raise ValueError("cameras_extent needs at least one camera")
     centers = np.stack([np.asarray(c["campos"], dtype=np.float64).reshape(3) for c in cams])
-    center = centers.mean(axis=0, keepdims=True)
-    return float(np.linalg.norm(centers - center, axis=1).max() * 1.1)
+    return float(nerfpp_radius(centers.T))
+
+
+def nerfpp_radius(cam_centers):
+    """The tail of getNerfppNorm (scene/dataset_readers.py:60-76) over (3, N) camera centres, in their dtype: the largest
+    distance from their mean, x 1.1.  numpy's reductions sum in an order set by the memory layout, so the bits depend
+    on it: the reference's np.hstack of (3, 1) columns is C-contiguous (scene.read_colmap_scene passes that), while
+    cameras_extent passes the transposed view of its (N, 3) rows."""
+    center = np.mean(cam_centers, axis=1, keepdims=True)
+    dist = np.linalg.norm(cam_centers - center, axis=0, keepdims=True)
+    return np.max(dist) * 1.1
