@@ -235,59 +235,102 @@ def preprocess_gaussians(means3D, scales, rotations, shs, opacities, raster_sett
                                       statlog.request(cuda_args))
 
 
-class _PreprocessGaussiansRaw(torch.autograd.Function):
-    """preprocess_gaussians with the GaussianModel activations fused in (gs_preprocess_*_raw)."""
+_RAW_NAMES = ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity")
+
+
+def _raw_camera(B, rs, cams):
+    """What the launch reads of the B views' cameras.  One view: (viewmatrix, projmatrix, campos, tanfovx, tanfovy), the
+    device matrices and host tangents the single-camera kernels take, from its settings rs or, without them, from the row
+    of the (1,40) table cams (the two tangents are read back to the host: a sync).  More views: the (B,40) device table
+    cams, or cams() when it is a callable (the table is then built only here)."""
+    if B == 1 and rs is not None:
+        return (_f32c(rs.viewmatrix, "viewmatrix"), _f32c(rs.projmatrix, "projmatrix"), _f32c(rs.campos, "campos"),
+                float(rs.tanfovx), float(rs.tanfovy))
+    cams = _f32c(cams() if callable(cams) else cams, "cams")
+    if tuple(cams.shape) != (B, 40):
+        raise ValueError(f"cams must be ({B},40) (pack_cameras), got {tuple(cams.shape)}")
+    if B > 1:
+        return cams
+    tanfovx, tanfovy = cams[0, 35:37].tolist()
+    return cams[0, :16], cams[0, 16:32], cams[0, 32:35], tanfovx, tanfovy
+
+
+def _launch_raw(direction, B, cam, P, meta, max_deg, params, *tail):
+    """gs_preprocess_{direction}_raw_sh (B = 1) or gs_preprocess_{direction}_batched_sh (B > 1); params: the six raw
+    parameters, tail: the direction's remaining tensors in the entry point's order."""
+    W, H, D, mod = meta
+    xyz, f_dc, f_rest, scaling, rotation, opacity = (t.data_ptr() for t in params)
+    body = (P, D, max_deg, xyz, f_dc, f_rest, scaling, mod, rotation, opacity)
+    tail = [t.data_ptr() for t in tail]
+    if B == 1:
+        vm, pm, cp, tanfovx, tanfovy = cam
+        _lib.call(f"gs_preprocess_{direction}_raw_sh", *body, vm.data_ptr(), pm.data_ptr(), cp.data_ptr(), W, H, tanfovx,
+                  tanfovy, *tail, _stream())
+    else:
+        _lib.call(f"gs_preprocess_{direction}_batched_sh", B, *body, cam.data_ptr(), W, H, *tail, _stream())
+
+
+class _PreprocessRaw(torch.autograd.Function):
+    """preprocess_gaussians' outputs for B views from the six RAW GaussianModel parameters
+    (scene/gaussian_model.py:219-228), the activations of :109-129 inside the kernel -> (means2D (B,P,2), rgb (B,P,3),
+    conic_opacity (B,P,4), radii (B,P) int32, depths (B,P)).  meta = (image_width, image_height, active sh_degree,
+    scale_modifier), shared by the views; rs, cams: the views' cameras (_raw_camera).
+
+    B > 1 is ONE batched launch over the (B,40) camera table, which reads every Gaussian once.  B = 1 launches the
+    single-camera kernels instead: both give equal outputs there, and the single-camera backward is the faster one,
+    0.357-0.361 ms for k_preprocess_bwd<true,16> against 0.410-0.413 ms for k_preprocess_bwd_batched<16> at c2
+    (DESIGN.md section 5)."""
 
     @staticmethod
-    def forward(ctx, xyz, f_dc, f_rest, scaling, rotation, opacity, rs):
+    def forward(ctx, xyz, f_dc, f_rest, scaling, rotation, opacity, B, rs, cams, meta):
         ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
-        xyz, f_dc, f_rest = _f32c(xyz, "_xyz"), _f32c(f_dc, "_features_dc"), _f32c(f_rest, "_features_rest")
-        scaling, rotation, opacity = _f32c(scaling, "_scaling"), _f32c(rotation, "_rotation"), _f32c(opacity, "_opacity")
         P = xyz.shape[0]
         if tuple(f_dc.shape) != (P, 1, 3) or f_rest.dim() != 3 or f_rest.shape[0] != P or f_rest.shape[2] != 3:
             raise ValueError("features must be (P,1,3) and (P,K-1,3) (scene/gaussian_model.py:219-228)")
-        max_deg = _stored_degree(f_rest.shape[1] + 1, rs.sh_degree, "_features_dc + _features_rest")
         if tuple(xyz.shape) != (P, 3) or tuple(scaling.shape) != (P, 3) or tuple(rotation.shape) != (P, 4) \
                 or opacity.numel() != P:
             raise ValueError("inconsistent Gaussian parameter shapes")
-        dev = xyz.device
-        vm, pm, cp = _f32c(rs.viewmatrix, "viewmatrix"), _f32c(rs.projmatrix, "projmatrix"), _f32c(rs.campos, "campos")
-        means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((P,), dev)
-        _lib.call("gs_preprocess_forward_raw_sh", P, int(rs.sh_degree), max_deg, xyz.data_ptr(), f_dc.data_ptr(),
-                  f_rest.data_ptr(), scaling.data_ptr(), float(rs.scale_modifier), rotation.data_ptr(),
-                  opacity.data_ptr(), vm.data_ptr(), pm.data_ptr(), cp.data_ptr(), int(rs.image_width),
-                  int(rs.image_height), float(rs.tanfovx), float(rs.tanfovy), means2D.data_ptr(), depths.data_ptr(),
-                  radii.data_ptr(), conic_opacity.data_ptr(), rgb.data_ptr(), clamped.data_ptr(), _stream())
-        ctx.rs, ctx.max_deg = rs, max_deg
-        ctx.cam = (vm, pm, cp)
-        ctx.save_for_backward(xyz, f_dc, f_rest, scaling, rotation, opacity, radii, clamped)
+        max_deg = _stored_degree(f_rest.shape[1] + 1, meta[2], "_features_dc + _features_rest")
+        params = [_f32c(t, name) for t, name in zip((xyz, f_dc, f_rest, scaling, rotation, opacity), _RAW_NAMES)]
+        cam = _raw_camera(B, rs, cams)
+        means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((B, P), xyz.device)
+        _launch_raw("forward", B, cam, P, meta, max_deg, params, means2D, depths, radii, conic_opacity, rgb, clamped)
+        ctx.cam, ctx.meta, ctx.max_deg = cam, meta, max_deg
+        ctx.save_for_backward(*params, radii, clamped)
         ctx.mark_non_differentiable(radii, depths)
         return means2D, rgb, conic_opacity, radii, depths
 
     @staticmethod
     def backward(ctx, g_means2D, g_rgb, g_conic_opacity, _g_radii, _g_depths):
-        xyz, f_dc, f_rest, scaling, rotation, opacity, radii, clamped = ctx.saved_tensors
-        rs = ctx.rs
-        vm, pm, cp = ctx.cam
-        P = xyz.shape[0]
-        dev = xyz.device
-        g_means2D, g_rgb = _grad_or_zeros(g_means2D, (P, 2), dev), _grad_or_zeros(g_rgb, (P, 3), dev)
-        g_conic_opacity = _grad_or_zeros(g_conic_opacity, (P, 4), dev)
-        d = [torch.empty_like(t) for t in (xyz, f_dc, f_rest, scaling, rotation, opacity)]
-        _lib.call("gs_preprocess_backward_raw_sh", P, int(rs.sh_degree), ctx.max_deg, xyz.data_ptr(), f_dc.data_ptr(),
-                  f_rest.data_ptr(), scaling.data_ptr(), float(rs.scale_modifier), rotation.data_ptr(),
-                  opacity.data_ptr(), vm.data_ptr(), pm.data_ptr(), cp.data_ptr(), int(rs.image_width),
-                  int(rs.image_height), float(rs.tanfovx), float(rs.tanfovy), radii.data_ptr(), clamped.data_ptr(),
-                  g_means2D.data_ptr(), g_conic_opacity.data_ptr(), g_rgb.data_ptr(), d[0].data_ptr(), d[1].data_ptr(),
-                  d[2].data_ptr(), d[3].data_ptr(), d[4].data_ptr(), d[5].data_ptr(), _stream())
-        return d[0], d[1], d[2], d[3], d[4], d[5], None
+        *params, radii, clamped = ctx.saved_tensors
+        B, P = radii.shape
+        grads = [_grad_or_zeros(g, (B, P, n), radii.device)
+                 for g, n in ((g_means2D, 2), (g_conic_opacity, 4), (g_rgb, 3))]
+        d = [torch.empty_like(t) for t in params]
+        _launch_raw("backward", B, ctx.cam, P, ctx.meta, ctx.max_deg, params, radii, clamped, *grads, *d)
+        return (*d, None, None, None, None)
 
 
 def preprocess_gaussians_raw(xyz, features_dc, features_rest, scaling, rotation, opacity, raster_settings):
     """Same outputs as preprocess_gaussians, from the six RAW GaussianModel parameters
     (scene/gaussian_model.py:219-228); the activations of :109-129 run inside the kernel.  features_rest (P,K-1,3),
-    (P,0,3) for a model stored at degree 0."""
-    return _PreprocessGaussiansRaw.apply(xyz, features_dc, features_rest, scaling, rotation, opacity, raster_settings)
+    (P,0,3) for a model stored at degree 0.  The one-view case of preprocess_gaussians_batched, with the camera read
+    from raster_settings."""
+    rs = raster_settings
+    out = _PreprocessRaw.apply(xyz, features_dc, features_rest, scaling, rotation, opacity, 1, rs, None,
+                               (int(rs.image_width), int(rs.image_height), int(rs.sh_degree), float(rs.scale_modifier)))
+    return tuple(t.squeeze(0) for t in out)
+
+
+def preprocess_gaussians_batched(xyz, features_dc, features_rest, scaling, rotation, opacity, cams, image_width,
+                                 image_height, sh_degree, scale_modifier=1.0):
+    """All B cameras at once from the RAW GaussianModel parameters (features_rest (P,K-1,3) as in
+    preprocess_gaussians_raw).  cams: pack_cameras(...) (B,40); at B = 1 its two tangents are read back to the host for
+    the single-camera kernels (a sync that preprocess_gaussians_raw, given the view's settings, does not need).
+    -> (means2D (B,P,2), rgb (B,P,3), conic_opacity (B,P,4), radii (B,P) int32, depths (B,P)); slice k equals the
+    single-camera operator's output for camera k."""
+    return _PreprocessRaw.apply(xyz, features_dc, features_rest, scaling, rotation, opacity, cams.shape[0], None, cams,
+                                (int(image_width), int(image_height), int(sh_degree), float(scale_modifier)))
 
 
 def deterministic_enabled(deterministic=None):
@@ -954,7 +997,7 @@ def merge_image_tiles_by_pos(all_pos_recv_from_i, all_tiles_recv_from_i, image_h
 
 
 # ---------------------------------------------------------------------------------------------------------
-# batched preprocess: all B cameras of a step in one launch
+# the camera table of preprocess_gaussians_batched
 # ---------------------------------------------------------------------------------------------------------
 def pack_cameras(settings_list):
     """(B,40) float32 device tensor: viewmatrix[16], projmatrix[16], campos[3], tanfovx, tanfovy, 3 pad per camera."""
@@ -965,54 +1008,3 @@ def pack_cameras(settings_list):
         rows.append(torch.cat([rs.viewmatrix.reshape(-1).float(), rs.projmatrix.reshape(-1).float(),
                                rs.campos.reshape(-1).float(), tail]))
     return torch.stack(rows).contiguous()
-
-
-class _PreprocessBatched(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, xyz, f_dc, f_rest, scaling, rotation, opacity, cams, meta):
-        ctx.set_materialize_grads(False)   # undefined output gradients arrive as None, not as zero-filled tensors
-        xyz, f_dc, f_rest = _f32c(xyz, "_xyz"), _f32c(f_dc, "_features_dc"), _f32c(f_rest, "_features_rest")
-        scaling, rotation, opacity = _f32c(scaling, "_scaling"), _f32c(rotation, "_rotation"), _f32c(opacity, "_opacity")
-        cams = _f32c(cams, "cams")
-        P, B = xyz.shape[0], cams.shape[0]
-        if tuple(f_dc.shape) != (P, 1, 3) or f_rest.dim() != 3 or f_rest.shape[0] != P or f_rest.shape[2] != 3 \
-                or cams.shape[1] != 40:
-            raise ValueError("features must be (P,1,3)/(P,K-1,3) and cams (B,40)")
-        W, H, D, mod = meta
-        max_deg = _stored_degree(f_rest.shape[1] + 1, D, "_features_dc + _features_rest")
-        dev = xyz.device
-        means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((B, P), dev)
-        _lib.call("gs_preprocess_forward_batched_sh", B, P, int(D), max_deg, xyz.data_ptr(), f_dc.data_ptr(),
-                  f_rest.data_ptr(), scaling.data_ptr(), float(mod), rotation.data_ptr(), opacity.data_ptr(),
-                  cams.data_ptr(), int(W), int(H), means2D.data_ptr(), depths.data_ptr(), radii.data_ptr(),
-                  conic_opacity.data_ptr(), rgb.data_ptr(), clamped.data_ptr(), _stream())
-        ctx.meta, ctx.max_deg = meta, max_deg
-        ctx.save_for_backward(xyz, f_dc, f_rest, scaling, rotation, opacity, cams, radii, clamped)
-        ctx.mark_non_differentiable(radii, depths)
-        return means2D, rgb, conic_opacity, radii, depths
-
-    @staticmethod
-    def backward(ctx, g_means2D, g_rgb, g_conic_opacity, _g_radii, _g_depths):
-        xyz, f_dc, f_rest, scaling, rotation, opacity, cams, radii, clamped = ctx.saved_tensors
-        W, H, D, mod = ctx.meta
-        P, B = xyz.shape[0], cams.shape[0]
-        dev = xyz.device
-        g_means2D, g_rgb = _grad_or_zeros(g_means2D, (B, P, 2), dev), _grad_or_zeros(g_rgb, (B, P, 3), dev)
-        g_conic_opacity = _grad_or_zeros(g_conic_opacity, (B, P, 4), dev)
-        d = [torch.empty_like(t) for t in (xyz, f_dc, f_rest, scaling, rotation, opacity)]
-        _lib.call("gs_preprocess_backward_batched_sh", B, P, int(D), ctx.max_deg, xyz.data_ptr(), f_dc.data_ptr(),
-                  f_rest.data_ptr(), scaling.data_ptr(), float(mod), rotation.data_ptr(), opacity.data_ptr(),
-                  cams.data_ptr(), int(W), int(H), radii.data_ptr(), clamped.data_ptr(), g_means2D.data_ptr(),
-                  g_conic_opacity.data_ptr(), g_rgb.data_ptr(), d[0].data_ptr(), d[1].data_ptr(), d[2].data_ptr(),
-                  d[3].data_ptr(), d[4].data_ptr(), d[5].data_ptr(), _stream())
-        return d[0], d[1], d[2], d[3], d[4], d[5], None, None
-
-
-def preprocess_gaussians_batched(xyz, features_dc, features_rest, scaling, rotation, opacity, cams, image_width,
-                                 image_height, sh_degree, scale_modifier=1.0):
-    """All B cameras at once from the RAW GaussianModel parameters (features_rest (P,K-1,3) as in
-    preprocess_gaussians_raw).  cams: pack_cameras(...) (B,40).
-    -> (means2D (B,P,2), rgb (B,P,3), conic_opacity (B,P,4), radii (B,P) int32, depths (B,P)); slice k equals the
-    single-camera operator's output for camera k."""
-    return _PreprocessBatched.apply(xyz, features_dc, features_rest, scaling, rotation, opacity, cams,
-                                    (int(image_width), int(image_height), int(sh_degree), float(scale_modifier)))

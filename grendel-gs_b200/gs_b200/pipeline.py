@@ -791,17 +791,12 @@ class Trainer:
 
     def _preprocess(self, rs, cam_table, B, training):
         """This rank's Gaussians projected into the B views of a batch -> (means2D (B,P,2), rgb, conic_opacity, radii,
-        depths).  One view runs the per-camera kernel with its settings rs, whose backward is faster than the batched
-        one's at B = 1 (DESIGN.md section 5); more run ONE batched launch over the (B,40) device camera table
-        cam_table(), which reads every Gaussian once.  training: means2D keeps its gradient, which
-        densification reads (means2D.grad of camera k, densification.py:24)."""
+        depths): a one-view batch with its settings rs, more over the (B,40) device camera table cam_table(), built only
+        then (ops._PreprocessRaw).  training: means2D keeps its gradient, which densification reads (means2D.grad of
+        camera k, densification.py:24)."""
         p = self.params
-        if B == 1:
-            out = tuple(t.unsqueeze(0) for t in ops.preprocess_gaussians_raw(
-                p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation, p._opacity, rs))
-        else:
-            out = ops.preprocess_gaussians_batched(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation,
-                                                   p._opacity, cam_table(), self.W, self.H, p.active_sh_degree)
+        out = ops._PreprocessRaw.apply(p._xyz, p._features_dc, p._features_rest, p._scaling, p._rotation, p._opacity, B,
+                                       rs, cam_table, (self.W, self.H, p.active_sh_degree, 1.0))
         if training:
             out[0].retain_grad()
         return out

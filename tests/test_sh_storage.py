@@ -1,7 +1,8 @@
 """CPU checks for models that store fewer SH coefficients (--sh_degree D < 3 in the reference: (D+1)^2 coefficients per
 Gaussian, scene/gaussian_model.py:51-53, 150-156): the _sh preprocess entry points and the width-parameterised sparse
-gradient rows refuse bad degrees, pointers and alignment before any launch, and redistribution moves the (P,0,3) and
-(P,3,3) _features_rest tensors of D = 0 and D = 1 models with their Adam moments."""
+gradient rows refuse bad degrees, pointers and alignment before any launch, the raw-parameter operators refuse
+inconsistent parameter shapes before any launch, and redistribution moves the (P,0,3) and (P,3,3) _features_rest tensors
+of D = 0 and D = 1 models with their Adam moments."""
 import json
 import os
 import subprocess
@@ -129,6 +130,35 @@ def test_scene_and_params_store_the_requested_degree():
         pipeline.GaussianParams(syn.make_scene(7, 64, 48, max_sh_degree=1), "cpu")     # 4 coefficients, degree 3 asked
     with pytest.raises(ValueError):
         pipeline.GaussianParams(full, "cpu", 4)
+
+
+def test_raw_operators_refuse_inconsistent_parameters_before_any_launch(monkeypatch):
+    """preprocess_gaussians_raw and preprocess_gaussians_batched (one view and two) check _xyz, _scaling, _rotation and
+    _opacity against the P rows of _xyz, and the features against P, before they read a camera or call the library: a
+    ValueError for each mismatch, here with tensors on the host that could not be launched anyway."""
+    from gs_b200 import _lib, ops, pipeline, synthetic as syn
+
+    def forbid(*_a, **_k):
+        raise AssertionError("the library was called")
+    monkeypatch.setattr(_lib, "call", forbid)
+    P, K = 5, 4
+    good = [torch.zeros(P, 3), torch.zeros(P, 1, 3), torch.zeros(P, K - 1, 3), torch.zeros(P, 3), torch.zeros(P, 4),
+            torch.zeros(P, 1)]
+    rs = pipeline.DeviceCamera(syn.make_camera(16, 16), "cpu").settings(1)
+    cases = [(0, (P, 4), "inconsistent"), (0, (P + 1, 3), "features"), (1, (P, 2, 3), "features"),
+             (2, (P + 1, K - 1, 3), "features"), (3, (P - 1, 3), "inconsistent"), (3, (P, 4), "inconsistent"),
+             (4, (P, 3), "inconsistent"), (4, (P + 1, 4), "inconsistent"), (5, (P + 1, 1), "inconsistent")]
+    for q, shape, msg in cases:
+        raw = list(good)
+        raw[q] = torch.zeros(shape)
+        with pytest.raises(ValueError, match=msg):
+            ops.preprocess_gaussians_raw(*raw, rs)
+        for B in (1, 2):
+            with pytest.raises(ValueError, match=msg):
+                ops.preprocess_gaussians_batched(*raw, torch.zeros(B, 40), 16, 16, 1)
+    for B in (1, 2):   # consistent parameters pass the checks and are refused only for living on the host
+        with pytest.raises(ValueError, match="CUDA tensor"):
+            ops.preprocess_gaussians_batched(*good, torch.zeros(B, 40), 16, 16, 1)
 
 
 def _redistribute_worker(rank, world, port, D, q):

@@ -251,6 +251,30 @@ def test_operators_take_the_stored_coefficients():
         ops.preprocess_gaussians_raw(*raw, pipeline.DeviceCamera(cam, gu.DEV).settings(4))
 
 
+@pytest.mark.parametrize("D_max", range(4))
+def test_batched_one_view_equals_the_single_camera_operator(D_max):
+    """preprocess_gaussians_batched over a one-view table == preprocess_gaussians_raw with that camera's settings, bit for
+    bit (-0 and +0 told apart): the five outputs and the six parameter gradients, for a model storing K = 1, 4, 9 or 16
+    coefficients.  Both run the single-camera kernels at B = 1."""
+    K, P, mod = _K(D_max), SIZES[-1], 0.8
+    cam, _, padded = _scene(D_max, D_max, P, 5 + D_max)
+    rs = pipeline.DeviceCamera(cam, gu.DEV).settings(D_max)
+    rs.scale_modifier = mod
+    gm, gc, gr = _grads(P, (P,), 6 + D_max)
+    res = []
+    for batched in (True, False):
+        raw = [t.clone().requires_grad_(True) for t in _raw_stored(gu.raw_parameters(padded), K)]
+        if batched:
+            out = [t[0] for t in ops.preprocess_gaussians_batched(*raw, ops.pack_cameras([rs]), W, H, D_max, mod)]
+        else:
+            out = ops.preprocess_gaussians_raw(*raw, rs)
+        ((out[0] * gm).sum() + (out[2] * gc).sum() + (out[1] * gr).sum()).backward()
+        res.append(([t.detach() for t in out], [t.grad for t in raw]))
+    assert int((res[1][0][3] > 0).sum()) > 1000
+    for q, (a, b) in enumerate(zip(res[0][0] + res[0][1], res[1][0] + res[1][1])):
+        assert bits_equal(a, b), (D_max, q)
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # a short training run: Trainer.step + FusedAdam, the active degree raised along the way, one densify_and_prune
 # ---------------------------------------------------------------------------------------------------------------------
