@@ -147,6 +147,36 @@ def train_step_single(params, dcam, gt_u8_dev, lambda_dssim=0.2, collector=None,
     return loss, means2D, radii
 
 
+def sum_over_ranks(gathered):
+    """(W, n, 2) per-rank [Ll1, ssim] records -> (n, 2): ((rank 0 + rank 1) + rank 2) + ..., in rank order, so the bits
+    depend only on which partial each rank holds, not on a collective's reduction order."""
+    total = gathered[0]
+    for r in range(1, gathered.shape[0]):
+        total = total + gathered[r]
+    return total
+
+
+def loss_table(gathered, index, lambda_dssim):
+    """The drained records as one table: (W, n, 2) gathered [Ll1, ssim] and (n,) camera indices -> (n, 4) float64 rows
+    (camera index, Ll1, ssim, loss).  loss = (1 - lambda) Ll1 + lambda (1 - ssim) in float32, as train_internal.py:220-222
+    forms batched_loss; the float32 values widen exactly."""
+    pairs = sum_over_ranks(gathered)
+    loss = (1.0 - lambda_dssim) * pairs[:, 0] + lambda_dssim * (1.0 - pairs[:, 1])
+    return torch.cat([index.to(torch.float64)[:, None], pairs.to(torch.float64), loss.to(torch.float64)[:, None]], 1)
+
+
+def loss_entries(rows, steps):
+    """loss_table's rows as host lists and the steps' (iteration, B), oldest first -> one entry per step:
+    {"iteration", "views", "l1", "ssim", "loss"}, the views' values in batch order."""
+    out, off = [], 0
+    for iteration, B in steps:
+        part = rows[off:off + B]
+        off += B
+        out.append({"iteration": int(iteration), "views": [int(r[0]) for r in part], "l1": [r[1] for r in part],
+                    "ssim": [r[2] for r in part], "loss": [r[3] for r in part]})
+    return out
+
+
 class Trainer:
     """Distributed training-step harness (one process per GPU).
 
@@ -295,6 +325,18 @@ class Trainer:
         self._loss_host = None
         self._info = {}
         self._h2d = 0
+        # per-view [Ll1, ssim] of every step since the last train_losses(): (slots, 2) fp32 and (slots,) int64 camera
+        # indices on the device, grown geometrically; the host keeps (iteration, B) per step.  Only local sampling at
+        # world size > 1 has batches whose camera indices the host does not know: the index buffer is filled then, and
+        # the host lists them (_rec_host_index) otherwise.
+        self._rec_pairs = self._rec_index = None
+        self._rec_used, self._rec_steps, self._rec_host_index = 0, [], []
+        self._rec_index_on_device = self.local_sampling and world > 1
+        # the border path's (1 - lambda, -lambda): a strip's loss is its [Ll1, ssim] dotted with it, plus lambda, the
+        # arithmetic of ops.fused_loss
+        lam = float(lambda_dssim)
+        self._loss_w = (torch.tensor([1.0 - lam, -lam], dtype=torch.float32, device=device)
+                        if border_exchange else None)
 
     @staticmethod
     def _model_total(model, shard, device, world, group):
@@ -383,7 +425,8 @@ class Trainer:
         order (a camera may appear more than once); None = all cameras in order.  The caller chooses them (the reference
         draws --bsz per step, train_internal.py:134).  resident=False copies the GT strips from pinned host memory inside
         the step and reads the loss back (the end-to-end leg); returns the loss as a float then.
-        With local_sampling, views are this rank's own local_bsz views (required)."""
+        With local_sampling, views are this rank's own local_bsz views (required).
+        Every step keeps its views' [Ll1, ssim] on the device for train_losses()."""
         views = self._local_views(views) if self.local_sampling else self._batch_views(views)
         ops.STEP_STREAM = torch.cuda.current_stream().cuda_stream   # every kernel of the step goes to this stream
         try:
@@ -430,6 +473,60 @@ class Trainer:
         args = self._eval_args("image_metrics", views, cams, gts, bsz)
         with self._eval_state():
             return self._image_metrics(*args, bool(images))
+
+    def train_losses(self):
+        """The training loss of every view of every step since the last call, as the reference reports it each step
+        (train_internal.py:211-238): per view [Ll1, ssim], both normalised by the full image's 3 H W, summed over the
+        ranks, and (1 - lambda) Ll1 + lambda (1 - ssim).  A collective, like evaluate: every rank calls it after the same
+        steps.  The steps' records are all-gathered in one all_gather_into_tensor (none at world size 1) and added in rank
+        order on the device (sum_over_ranks), so the bits depend on the strip division only, not on NCCL's reduction
+        order; one host read.  The records are then cleared.
+        -> one entry per step, oldest first: {"iteration": the step's number (Trainer.iteration after it), "views": its
+        camera indices in batch order, "l1", "ssim", "loss": lists of floats, one per view}; [] when no step is pending."""
+        n = self._rec_used
+        if n == 0:
+            return []
+        mine = self._rec_pairs[:n]
+        if self.world > 1:
+            import torch.distributed as dist
+            allp = torch.empty((self.world * n, 2), dtype=torch.float32, device=self.device)
+            dist.all_gather_into_tensor(allp, mine, group=self.group)
+            gathered = allp.reshape(self.world, n, 2)
+        else:
+            gathered = mine[None]
+        steps = self._rec_steps
+        if self._rec_index_on_device:
+            index = self._rec_index[:n]
+        else:
+            index = torch.tensor(self._rec_host_index, dtype=torch.int64).to(self.device)
+        rows = loss_table(gathered, index, self.lambda_dssim).tolist()   # the call's one host read
+        mine.zero_()   # unused slots stay +0.0 for the positions a later step has no strip of
+        self._rec_used, self._rec_steps, self._rec_host_index = 0, [], []
+        return loss_entries(rows, steps)
+
+    def _record_losses(self, views, B, span=None, l1_ssim=None, strips=()):
+        """Keep this step's (B, 2) [Ll1, ssim] in batch-position order: the span (lo, hi) of l1_ssim, or (k, (1,2) pair)
+        per local strip; every other position stays +0.0.  Device copies into the record buffer, no host sync.  The
+        camera indices stay on the host when it knows the batch; under local sampling at world size > 1 they are copied
+        from the device-gathered batch index."""
+        off = self._rec_used
+        if self._rec_pairs is None or off + B > self._rec_pairs.shape[0]:
+            cap = max(256, 2 * (0 if self._rec_pairs is None else self._rec_pairs.shape[0]), off + B)
+            pairs = torch.zeros((cap, 2), dtype=torch.float32, device=self.device)
+            index = torch.zeros((cap,), dtype=torch.int64, device=self.device)
+            if off:
+                pairs[:off].copy_(self._rec_pairs[:off]); index[:off].copy_(self._rec_index[:off])
+            self._rec_pairs, self._rec_index = pairs, index
+        if l1_ssim is not None:
+            self._rec_pairs[off + span[0]:off + span[1]].copy_(l1_ssim.detach())
+        for k, pair in strips:
+            self._rec_pairs[off + k].copy_(pair.detach().reshape(2))
+        if self._rec_index_on_device:
+            self._rec_index[off:off + B].copy_(self._batch_index)
+        else:
+            self._rec_host_index.extend(views)
+        self._rec_used = off + B
+        self._rec_steps.append((self.iteration + 1, B))
 
     def _eval_args(self, name, views, cams, gts, bsz):
         """The refusals of evaluate / image_metrics, from the arguments alone, before any collective or launch.
@@ -725,8 +822,10 @@ class Trainer:
         self.means2D, self._radii_local = fw.means2D, fw.radii
         if self.border_exchange:
             # the legacy row L1: one loss per local strip, summed in view order; a strip of a view split over several
-            # ranks is widened by the 5 halo rows its neighbours render, so the strip losses sum to the full-image loss
-            loss_sum = None
+            # ranks is widened by the 5 halo rows its neighbours render, so the strip losses sum to the full-image loss.
+            # Each strip's [Ll1, ssim] is kept for the record; its loss is ops.fused_loss's arithmetic on it (the same
+            # launch, dot with (1 - lambda, -lambda), + lambda), so the loss and gradients keep their bits.
+            loss_sum, pairs = None, []
             for k, st in enumerate(strategies):
                 rows = st.local_pixel_rows(self.H)
                 if rows is None:
@@ -734,13 +833,17 @@ class Trainer:
                 if len(st.gpu_ids) > 1:
                     from . import border
                     image, (r0, r1), _ = border.add_remote_border_rows(fw.images[k], st, self.H, self.group)
-                    loss = ops.fused_loss(image, self.gts_dev[views[k]], r0, r1, self.lambda_dssim, *rows,
-                                          deterministic=self.deterministic, gt_full=True)
+                    gt, rows4, gt_full = self.gts_dev[views[k]], (r0, r1, *rows), True
                 else:
+                    image, rows4 = fw.images[k], (*rows, *rows)
                     gt = self.gts_dev[views[k]] if resident else self._wait_gt(gt_ready[k])
-                    loss = ops.fused_loss(fw.images[k], gt, *rows, self.lambda_dssim, deterministic=self.deterministic,
-                                          gt_full=resident and rows != (0, self.H))
+                    gt_full = resident and rows != (0, self.H)
+                pair = ops.fused_l1_ssim_batched(image[None], [gt], [rows4], deterministic=self.deterministic,
+                                                 gt_full=gt_full)
+                pairs.append((k, pair))
+                loss = torch.dot(pair.reshape(-1), self._loss_w) + float(self.lambda_dssim)
                 loss_sum = loss if loss_sum is None else loss_sum + loss
+            self._record_losses(views, len(strategies), strips=pairs)
         else:
             gts = [None if y1 == y0 else self.gts_dev[views[k]] if resident else self._wait_gt(gt_ready[k])
                    for k, (y0, y1, _c0, _c1) in enumerate(fw.rows4)]
@@ -751,6 +854,7 @@ class Trainer:
                                                 gt_full=gt_full)
             # sum over the local strips of (1 - lambda) Ll1 + lambda (1 - ssim)
             loss_sum = torch.dot(l1_ssim.reshape(-1), fw.coef) + fw.const
+            self._record_losses(views, len(strategies), span=(lo, hi), l1_ssim=l1_ssim)
         self._mark("r render+loss")
         loss_sum.backward()
         self._mark("b4 backward (rest)")

@@ -1,4 +1,5 @@
-"""The reference's --zhx_time / --zhx_debug log files, written by the drop-in operators on logging iterations.
+"""The reference's --zhx_time / --zhx_debug log files, written by the drop-in operators on logging iterations, and the
+training log's loss lines (train_loss_text, EpochLoss), written by the caller from Trainer.train_losses().
 
 The reference hands every rasterizer call a `cuda_args` dict of strings (gaussian_renderer/__init__.py:510-539).  Its
 CUDA extension appends, on logging iterations, to files in cuda_args["log_folder"] that analyze_statistic.py parses:
@@ -81,6 +82,39 @@ def n_contrib_text(iteration, local_rank, world_size, image_height, image_width,
                  f"global_ave_n_considered_per_pix: {int(ts[local, 1].sum()) / num_pixels:.6f}, "
                  f"global_ave_n_contrib2loss_per_pix: {int(ts[local, 2].sum()) / num_pixels:.6f}\n")
     return "".join(lines)
+
+
+def train_loss_text(iteration, bsz, losses, names):
+    """The training log's line of one step (train_internal.py:229-236): `iteration[{it},{it+bsz}) loss: [l0, ...] image:
+    ['name0', ...]`, each loss rounded to 6 places.  The losses are written as plain Python floats so that the parser's
+    float() reads each one (draw_iteration_loss, analyze_statistic.py:2765-2790); names are the views' image names, in
+    batch order."""
+    it = int(iteration)
+    return "iteration[{},{}) loss: {} image: {}\n".format(it, it + int(bsz), [round(float(v), 6) for v in losses],
+                                                         [str(n) for n in names])
+
+
+class EpochLoss:
+    """SceneDataset.update_losses (scene/__init__.py:284-295): the per-view losses in the order they came; after every
+    camera_size of them, `epoch {n} loss: {mean}` (parsed by draw_epoch_loss, analyze_statistic.py:2746-2755).  The mean
+    is a Python float sum over camera_size."""
+
+    def __init__(self, camera_size):
+        if int(camera_size) < 1:
+            raise ValueError(f"camera_size must be positive, got {camera_size}")
+        self.camera_size = int(camera_size)
+        self.iteration_loss, self.epoch_loss = [], []
+
+    def update(self, losses):
+        """Take one step's losses -> the text of the epoch lines they complete ("" when none)."""
+        lines = []
+        for v in losses:
+            self.iteration_loss.append(float(v))
+            if len(self.iteration_loss) % self.camera_size == 0:
+                self.epoch_loss.append(sum(self.iteration_loss[-self.camera_size:]) / self.camera_size)
+                lines.append(f"epoch {len(self.epoch_loss)} loss: {self.epoch_loss[-1]}\n")
+                self.iteration_loss = []
+        return "".join(lines)
 
 
 def append(path, text):
