@@ -278,3 +278,49 @@ extern "C" int gs_densify_stats(int num_views, int P, const void *const *grad_ho
     GS_LAUNCH_CHECK();
     return GS_OK;
 }
+
+// Opacity reset (scene/gaussian_model.py:555-561 with replace_tensor_to_optimizer :771-787):
+//     o = inverse_sigmoid(torch.min(sigmoid(o), ones_like * 0.01));  exp_avg = exp_avg_sq = 0
+// in torch's CUDA arithmetic, one rounding per operation: sigmoid is 1 / (1 + expf(-o)), ones * 0.01 is 0.01f, min
+// returns a NaN operand, inverse_sigmoid is logf(m / (1 - m)).  Every element takes the round trip (logit of a
+// sigmoid is not the identity in fp32), at or below 0.01 too.
+GS_D float ro_reset(float o) {
+    const float s = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-o)));
+    const float m = (isnan(s) || s < 0.01f) ? s : 0.01f;
+    return logf(__fdiv_rn(m, __fsub_rn(1.f, m)));
+}
+
+__global__ void __launch_bounds__(DN_THREADS)
+k_reset_opacity(long long P, float *__restrict__ o, float *__restrict__ m, float *__restrict__ v, int vec) {
+    const long long base = ((long long)blockIdx.x * DN_THREADS + threadIdx.x) * 4;
+    if (base >= P) return;
+    if (vec && base + 4 <= P) {
+        float4 x = *reinterpret_cast<float4 *>(o + base);
+        x.x = ro_reset(x.x); x.y = ro_reset(x.y); x.z = ro_reset(x.z); x.w = ro_reset(x.w);
+        *reinterpret_cast<float4 *>(o + base) = x;
+        if (m) {
+            *reinterpret_cast<float4 *>(m + base) = make_float4(0.f, 0.f, 0.f, 0.f);
+            *reinterpret_cast<float4 *>(v + base) = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        return;
+    }
+    const int cnt = (int)min(4ll, P - base);
+    for (int q = 0; q < cnt; q++) {
+        o[base + q] = ro_reset(o[base + q]);
+        if (m) { m[base + q] = 0.f; v[base + q] = 0.f; }
+    }
+}
+
+extern "C" int gs_reset_opacity(int P, float *opacity_raw, float *exp_avg, float *exp_avg_sq, void *stream) {
+    GS_REQUIRE(P >= 0, "P");
+    GS_REQUIRE(!exp_avg == !exp_avg_sq, "exp_avg and exp_avg_sq: both or neither");
+    if (P == 0) return GS_OK;
+    GS_REQUIRE(opacity_raw, "null pointer");
+    const uintptr_t all = (uintptr_t)opacity_raw | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq;
+    GS_REQUIRE((all & 3) == 0, "tensors must be 4-byte aligned");
+    const long long per_block = (long long)DN_THREADS * 4;
+    k_reset_opacity<<<(unsigned)((P + per_block - 1) / per_block), DN_THREADS, 0, (cudaStream_t)stream>>>(
+        P, opacity_raw, exp_avg, exp_avg_sq, (all & 15) == 0 ? 1 : 0);
+    GS_LAUNCH_CHECK();
+    return GS_OK;
+}

@@ -119,6 +119,7 @@ SIGNATURES = {
     "gs_densify_select": (_i, [_i, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _real, _real, _i, _vp, _sz, _vp, _vp]),
     "gs_densify_gather": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gs_densify_stats": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gs_reset_opacity": (_i, [_i, _vp, _vp, _vp, _vp]),
     "gs_peer_alloc": (_i, [_sz, C.POINTER(C.c_void_p), _vp]),
     "gs_peer_open": (_i, [_vp, C.POINTER(C.c_void_p)]),
     "gs_peer_close": (_i, [_vp]),

@@ -110,6 +110,35 @@ def densify_and_prune(optimizer, xyz_gradient_accum, denom, max_grad, min_opacit
     return result
 
 
+def reset_opacity(optimizer):
+    """GaussianModel.reset_opacity with replace_tensor_to_optimizer (scene/gaussian_model.py:555-561, :771-787), in
+    place, one launch (gs_reset_opacity): every opacity logit o becomes inverse_sigmoid(min(sigmoid(o), 0.01)) and both
+    Adam moments of the "opacity" group become zero, bit for bit as the reference's torch on the device; "step" is kept.
+    The reference puts a NEW Parameter without a gradient into the group, so the optimizer step of that iteration skips
+    the opacity; here the same parameter is kept and its .grad is set to None, which has that effect.
+    -> the opacity parameter."""
+    groups = {g["name"]: g for g in optimizer.param_groups}
+    if "opacity" not in groups or len(groups["opacity"]["params"]) != 1:
+        raise ValueError("the optimizer needs the reference's single-tensor \"opacity\" group")
+    p = groups["opacity"]["params"][0]
+    _check(p.data, "opacity", torch.float32, (None, 1))
+    if not p.is_cuda:
+        raise TypeError("reset_opacity needs a CUDA tensor (no CPU path)")
+    st = optimizer.state.get(p, None)
+    m = v = None
+    if st is not None and "exp_avg" in st:
+        m, v = st["exp_avg"], st["exp_avg_sq"]
+        for name, t in (("exp_avg", m), ("exp_avg_sq", v)):
+            _check(t, name, torch.float32, tuple(p.shape))
+            if t.device != p.device:
+                raise ValueError("the opacity moments must be on the parameter's device")
+    with torch.cuda.device(p.device):
+        _lib.call("gs_reset_opacity", p.shape[0], p.data.data_ptr(), m.data_ptr() if m is not None else None,
+                  v.data_ptr() if v is not None else None, torch.cuda.current_stream(p.device).cuda_stream)
+    p.grad = None
+    return p
+
+
 def _check(t, name, dtype, shape):
     """Refuse anything but a contiguous tensor of `dtype` and `shape` (None in `shape`: any size)."""
     if t is None:

@@ -649,6 +649,13 @@ GS_API int gs_densify_gather(int P, int S, int new_P, int num_tensors, const voi
  * updated in place.  One launch, no atomics, no host synchronisation; P == 0 launches nothing. */
 GS_API int gs_densify_stats(int num_views, int P, const void *const *grad_host, const void *const *radii_host,
                             float *xyz_gradient_accum, float *denom, float *max_radii2D, void *stream);
+/* Opacity reset (scene/gaussian_model.py:555-561 with replace_tensor_to_optimizer :771-787), in place, one launch:
+ *     opacity_raw[i] = log(m / (1 - m)),  m = min(sigmoid(opacity_raw[i]), 0.01f)      (every i, no skip)
+ *     exp_avg[i] = exp_avg_sq[i] = 0
+ * in torch's CUDA fp32 arithmetic (sigmoid 1 / (1 + expf(-x)), min propagating NaN), bit for bit.  The step counter is
+ * the caller's and is not touched.  P fp32 elements each, 4-byte aligned (float4 when all are 16-byte aligned);
+ * exp_avg and exp_avg_sq are both NULL (no optimizer state yet: only the opacity is written) or both set. */
+GS_API int gs_reset_opacity(int P, float *opacity_raw, float *exp_avg, float *exp_avg_sq, void *stream);
 
 /* ---- simple_knn._C.distCUDA2 -- /root/reference/scene/gaussian_model.py:20,163-166 ------------------------------------
  * Mean squared distance of every point to its 3 nearest OTHER points (self excluded by index, duplicates count at
