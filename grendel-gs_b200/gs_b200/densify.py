@@ -1,24 +1,22 @@
 """Densification step on top of gs_densify_select / gs_densify_gather: the effect of GaussianModel.densify_and_prune
 (/root/reference/scene/gaussian_model.py:1005-1044 -> densify_and_clone :973-1003, densify_and_split :922-971,
 densification_postfix :884-920, cat_tensors_to_optimizer :837-881, prune_points :816-835, _prune_optimizer :789-814) on
-an optimizer with the reference's six single-tensor groups ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation"):
-three launches and one host read-back instead of ~150 torch kernels and a dozen read-backs.
+an optimizer with the reference's six single-tensor groups (optim.NAMES): three launches and one host read-back
+instead of ~150 torch kernels and a dozen read-backs.
 
-The optimizer is edited the way the reference edits it: every group gets a NEW nn.Parameter, its state entry moves to
-the new parameter with exp_avg / exp_avg_sq replaced (survivors keep their moments, new Gaussians start at zero) and
-"step" untouched.  No CPU path.  The algorithm is checked on CPU against the reference's own run
+The optimizer is edited the way the reference edits it (optim.swap_rows): survivors keep their moments, new Gaussians
+start at zero and "step" is untouched.  No CPU path.  The algorithm is checked on CPU against the reference's own run
 (tests/test_densify_oracle.py) and on the device, decision for decision and bit for bit, against the reference's chain
 of torch operations run on the same device (tests/test_densify_gpu.py).
 """
 import ctypes as C
 
 import torch
-import torch.nn as nn
 
 from . import _lib
 from .ops import MAX_VIEWS
+from .optim import NAMES, group_param, group_params, moments, swap_rows
 
-NAMES = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation")
 KIND = {"xyz": 1, "scaling": 2}   # 0 copy, 1 position, 2 log-scale, 3 Adam moment (include/grendel_gs_b200.h)
 
 
@@ -38,10 +36,7 @@ def densify_and_prune(optimizer, xyz_gradient_accum, denom, max_grad, min_opacit
     "max_radii2D", "sum_visible_count_in_one_batch"), "send_to_gpui_cnt" (if given) and "counts" = (kept, clones,
     children per copy, split-selected, new total).  `noise`: optional (>= 2 S, 3) standard-normal draws for the split
     (default: torch.randn on the device, like the reference's torch.normal)."""
-    groups = {g["name"]: g for g in optimizer.param_groups}
-    if set(groups) != set(NAMES) or any(len(g["params"]) != 1 for g in groups.values()):
-        raise ValueError("the optimizer must have the reference's six single-tensor groups " + str(NAMES))
-    params = {k: groups[k]["params"][0] for k in NAMES}
+    params = group_params(optimizer)
     P = params["xyz"].shape[0]
     dev = params["xyz"].device
     if P == 0:
@@ -74,13 +69,12 @@ def densify_and_prune(optimizer, xyz_gradient_accum, denom, max_grad, min_opacit
             return
         src.append(t); dst.append(o); width.append(w); kind.append(k)
 
+    state = {k: moments(optimizer, p) for k, p in params.items()}
     with torch.no_grad():
         for k in NAMES:
             add(k, params[k].detach(), KIND.get(k, 0))
-            st = optimizer.state.get(params[k], None)
-            if st is not None and "exp_avg" in st:
-                add(k + ".exp_avg", st["exp_avg"], 3)
-                add(k + ".exp_avg_sq", st["exp_avg_sq"], 3)
+            for j, t in enumerate(state[k] or ()):
+                add((k, j), t, 3)
         if send_to_gpui_cnt is not None:
             add("send_to_gpui_cnt", send_to_gpui_cnt, 0)
         n = len(src)
@@ -88,22 +82,8 @@ def densify_and_prune(optimizer, xyz_gradient_accum, denom, max_grad, min_opacit
         _lib.call("gs_densify_gather", P, S, new_P, n, vp(*[t.data_ptr() for t in src]), vp(*[t.data_ptr() for t in dst]),
                   i32(*width), i32(*kind), params["scaling"].data_ptr(), params["rotation"].data_ptr(), noise.data_ptr(),
                   temp.data_ptr(), stream)
-    # move the optimizer over to the new tensors (gaussian_model.py:789-814 / :837-881)
-    result = {}
-    for k in NAMES:
-        g, old = groups[k], params[k]
-        new = nn.Parameter(outs[k].requires_grad_(True))
-        st = optimizer.state.pop(old, None)
-        if st is not None:
-            if "exp_avg" in st:
-                st["exp_avg"], st["exp_avg_sq"] = outs[k + ".exp_avg"], outs[k + ".exp_avg_sq"]
-            optimizer.state[new] = st
-        g["params"][0] = new
-        result[k] = new
-    result["xyz_gradient_accum"] = torch.zeros((new_P, 1), device=dev)          # densification_postfix :909-914
-    result["denom"] = torch.zeros((new_P, 1), device=dev)
-    result["max_radii2D"] = torch.zeros((new_P,), device=dev)
-    result["sum_visible_count_in_one_batch"] = torch.zeros((new_P,), device=dev)
+    result = swap_rows(optimizer, {k: (outs[k], None if state[k] is None else (outs[k, 0], outs[k, 1])) for k in NAMES})
+    result.update(fresh_stats(new_P, dev))          # densification_postfix :909-914
     if send_to_gpui_cnt is not None:
         result["send_to_gpui_cnt"] = outs["send_to_gpui_cnt"]
     result["counts"] = (kept, clones, child1, S, new_P)
@@ -117,18 +97,13 @@ def reset_opacity(optimizer):
     The reference puts a NEW Parameter without a gradient into the group, so the optimizer step of that iteration skips
     the opacity; here the same parameter is kept and its .grad is set to None, which has that effect.
     -> the opacity parameter."""
-    groups = {g["name"]: g for g in optimizer.param_groups}
-    if "opacity" not in groups or len(groups["opacity"]["params"]) != 1:
-        raise ValueError("the optimizer needs the reference's single-tensor \"opacity\" group")
-    p = groups["opacity"]["params"][0]
+    p = group_param(optimizer, "opacity")
     _check(p.data, "opacity", torch.float32, (None, 1))
     if not p.is_cuda:
         raise TypeError("reset_opacity needs a CUDA tensor (no CPU path)")
-    st = optimizer.state.get(p, None)
-    m = v = None
-    if st is not None and "exp_avg" in st:
-        m, v = st["exp_avg"], st["exp_avg_sq"]
-        for name, t in (("exp_avg", m), ("exp_avg_sq", v)):
+    m, v = moments(optimizer, p) or (None, None)
+    if m is not None:
+        for name, t in (("the opacity's first moment", m), ("the opacity's second moment", v)):
             _check(t, name, torch.float32, tuple(p.shape))
             if t.device != p.device:
                 raise ValueError("the opacity moments must be on the parameter's device")
@@ -195,18 +170,19 @@ def add_densification_stats(xyz_gradient_accum, denom, max_radii2D, means2D_grad
 def append_gaussians(optimizer, new_tensors):
     """cat_tensors_to_optimizer (/root/reference/scene/gaussian_model.py:837-881): rows appended to every parameter, their
     Adam moments start at zero, "step" is kept.  new_tensors: {group name: (n, ...) tensor}.  -> {name: new Parameter}."""
-    groups = {g["name"]: g for g in optimizer.param_groups}
-    out = {}
+    new = {}
     for k in NAMES:
-        g = groups[k]
-        old, ext = g["params"][0], new_tensors[k].to(device=g["params"][0].device, dtype=g["params"][0].dtype)
-        new = nn.Parameter(torch.cat((old.detach(), ext), dim=0).contiguous().requires_grad_(True))
-        st = optimizer.state.pop(old, None)
-        if st is not None:
-            if "exp_avg" in st:
-                st["exp_avg"] = torch.cat((st["exp_avg"], torch.zeros_like(ext)), dim=0)
-                st["exp_avg_sq"] = torch.cat((st["exp_avg_sq"], torch.zeros_like(ext)), dim=0)
-            optimizer.state[new] = st
-        g["params"][0] = new
-        out[k] = new
-    return out
+        old = group_param(optimizer, k)
+        ext = new_tensors[k].to(device=old.device, dtype=old.dtype)
+        m = moments(optimizer, old)
+        new[k] = (torch.cat((old.detach(), ext), dim=0),
+                  None if m is None else tuple(torch.cat((t, torch.zeros_like(ext)), dim=0) for t in m))
+    return swap_rows(optimizer, new)
+
+
+def fresh_stats(n, device):
+    """The per-Gaussian densification statistics of n Gaussians right after the model changed (densification_postfix,
+    scene/gaussian_model.py:909-914): all zero."""
+    return {"xyz_gradient_accum": torch.zeros((n, 1), device=device), "denom": torch.zeros((n, 1), device=device),
+            "max_radii2D": torch.zeros((n,), device=device),
+            "sum_visible_count_in_one_batch": torch.zeros((n,), device=device)}

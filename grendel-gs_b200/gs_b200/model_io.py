@@ -22,14 +22,13 @@ import torch
 import torch.distributed as dist
 
 from .exchange import all_to_all_single
-from .pipeline import Trainer
+from .optim import GROUPS, NAMES, FusedAdam, group_params
 from .redistribute import fused_rows
 
-# the capture() order of the six parameters (gaussian_model.py:70-84) differs from the optimizer's group order
+# the capture() order of the six parameters (gaussian_model.py:70-84), the checkpoint tuple's, is not the group order
 CAPTURE_NAMES = ("xyz", "f_dc", "f_rest", "scaling", "rotation", "opacity")
 STAT_NAMES = ("max_radii2D", "xyz_gradient_accum", "denom")
-ATTR = Trainer.GROUP_OF                 # group name -> GaussianParams attribute
-GROUP_ORDER = tuple(Trainer.GROUP_OF)   # the optimizer's groups, gaussian_model.py:257-292
+ATTR, GROUP_ORDER = GROUPS, NAMES   # group name -> GaussianParams attribute; the optimizer's group order
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -47,13 +46,6 @@ def ply_header(n, max_sh_degree):
     """The header plyfile writes for PlyData([PlyElement.describe(elements, "vertex")]) of n float rows."""
     props = "".join(f"property float {a}\n" for a in attribute_names(max_sh_degree))
     return f"ply\nformat binary_little_endian 1.0\nelement vertex {int(n)}\n{props}end_header\n".encode("ascii")
-
-
-def _degree_of(params):
-    km1 = params["f_rest"].shape[1]
-    if params["f_rest"].dim() != 3 or km1 + 1 not in (1, 4, 9, 16):
-        raise ValueError(f"f_rest must be (P, (D+1)^2 - 1, 3) for D = 0..3, got {tuple(params['f_rest'].shape)}")
-    return int(round((km1 + 1) ** 0.5)) - 1
 
 
 def ply_rows(params):
@@ -262,9 +254,8 @@ def save_ply(folder, trainer, gather=False):
     as one PLY row per Gaussian in ONE all_to_all_single in which only rank 0 receives, sized by one all-gather (the
     reference: six tensors, each with W - 1 send / recv pairs).  Returns the path written on this rank, or None."""
     rank, world, group = trainer.rank, trainer.world, trainer.group
-    params = _raw_of(trainer)
-    D = _degree_of(params)
-    rows = ply_rows(params)
+    D = trainer.params.max_sh_degree   # write_ply refuses rows of another degree
+    rows = ply_rows(_raw_of(trainer))
     if not gather:
         os.makedirs(folder, exist_ok=True)
         path = os.path.join(folder, f"point_cloud_rk{rank}_ws{world}.ply")
@@ -361,12 +352,9 @@ def save_checkpoint(folder, trainer, optimizer, stats, next_iteration, spatial_l
     torch.optim.Adam); stats: {"max_radii2D", "xyz_gradient_accum", "denom"}, the densification statistics the caller
     keeps.  The file loads into the reference's restore() and torch.optim.Adam.  -> the path written."""
     params = _raw_of(trainer)
-    names = [g.get("name") for g in optimizer.param_groups]
-    if names != list(GROUP_ORDER):
-        raise ValueError(f"the optimizer must have the reference's six groups in the order {GROUP_ORDER}, got {names}")
-    for g in optimizer.param_groups:
-        if len(g["params"]) != 1 or g["params"][0] is not params[g["name"]]:
-            raise ValueError(f"optimizer group {g['name']!r} does not hold the trainer's parameter (adopt_parameters "
+    for k, p in group_params(optimizer, ordered=True).items():
+        if p is not params[k]:
+            raise ValueError(f"optimizer group {k!r} does not hold the trainer's parameter (adopt_parameters "
                              "after densification or redistribution)")
     P = int(params["xyz"].shape[0])
     for k in STAT_NAMES:
@@ -480,12 +468,9 @@ def load_fused_adam(trainer, checkpoint, **kw):
     """A FusedAdam over trainer.optimizer_groups() with the checkpoint's optimizer state loaded (learning rates, betas,
     eps, step and moments: the saved groups replace the new ones, as torch.optim's load_state_dict does).  The groups
     must be the reference's six, in its order.  kw: FusedAdam's constructor arguments (grad_scale)."""
-    from .optim import FusedAdam
-    saved = [g.get("name") for g in checkpoint.optimizer_state["param_groups"]]
-    if saved != list(GROUP_ORDER):
-        raise ValueError(f"the checkpoint's optimizer groups are {saved}, expected {list(GROUP_ORDER)}")
     opt = FusedAdam(trainer.optimizer_groups(), lr=0.0, eps=1e-15, **kw)
     opt.load_state_dict(checkpoint.optimizer_state)
+    group_params(opt, ordered=True)   # the saved groups, which replaced the new ones
     for st in opt.state.values():   # the step counter lives on the host, as FusedAdam creates it
         if "step" in st:
             st["step"] = torch.as_tensor(st["step"], dtype=torch.float32).cpu()

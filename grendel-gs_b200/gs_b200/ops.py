@@ -111,12 +111,16 @@ def _screen_outputs(lead, dev):
 _STORED_DEGREE = {1: 0, 4: 1, 9: 2, 16: 3}
 
 
-def _stored_degree(K, sh_degree, what):
-    """max_sh_degree of a model storing K SH coefficients; ValueError (before any launch) for any other K or for an active
-    sh_degree outside 0..max_sh_degree."""
+def stored_sh_degree(K, what):
+    """max_sh_degree of a model storing K SH coefficients per Gaussian; ValueError naming `what` for any other K."""
     if K not in _STORED_DEGREE:
         raise ValueError(f"{what}: a model stores (D+1)^2 SH coefficients, D = 0..3 (1, 4, 9 or 16), got {K}")
-    D = _STORED_DEGREE[K]
+    return _STORED_DEGREE[K]
+
+
+def _stored_degree(K, sh_degree, what):
+    """stored_sh_degree, and a ValueError (before any launch) for an active sh_degree outside 0..max_sh_degree."""
+    D = stored_sh_degree(K, what)
     if not 0 <= int(sh_degree) <= D:
         raise ValueError(f"active sh_degree {sh_degree} is outside 0..{D}, the degree the model stores ({K} coefficients)")
     return D
@@ -235,7 +239,8 @@ def preprocess_gaussians(means3D, scales, rotations, shs, opacities, raster_sett
                                       statlog.request(cuda_args))
 
 
-_RAW_NAMES = ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity")
+# the raw preprocess operator's argument order, the C ABI's (GaussianParams attributes; GaussianParams.raw_parameters)
+RAW_ORDER = ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity")
 
 
 def _raw_camera(B, rs, cams):
@@ -291,7 +296,7 @@ class _PreprocessRaw(torch.autograd.Function):
                 or opacity.numel() != P:
             raise ValueError("inconsistent Gaussian parameter shapes")
         max_deg = _stored_degree(f_rest.shape[1] + 1, meta[2], "_features_dc + _features_rest")
-        params = [_f32c(t, name) for t, name in zip((xyz, f_dc, f_rest, scaling, rotation, opacity), _RAW_NAMES)]
+        params = [_f32c(t, name) for t, name in zip((xyz, f_dc, f_rest, scaling, rotation, opacity), RAW_ORDER)]
         cam = _raw_camera(B, rs, cams)
         means2D, depths, radii, conic_opacity, rgb, clamped = _screen_outputs((B, P), xyz.device)
         _launch_raw("forward", B, cam, P, meta, max_deg, params, means2D, depths, radii, conic_opacity, rgb, clamped)

@@ -11,10 +11,58 @@ mode, :295-312): same constructor, same `param_groups`, and the SAME state layou
 import ctypes as C
 
 import torch
+import torch.nn as nn
 
 from . import _lib
 
 MAX_TENSORS = 8   # GS_ADAM_MAX_TENSORS
+
+# the optimizer's groups in the reference's order (scene/gaussian_model.py:257-292): group name -> GaussianParams attribute
+GROUPS = {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity",
+          "scaling": "_scaling", "rotation": "_rotation"}
+NAMES = tuple(GROUPS)
+
+
+def group_param(optimizer, name):
+    """The parameter of the optimizer's single-tensor group `name`; ValueError unless there is exactly one such group."""
+    found = [g["params"] for g in optimizer.param_groups if g.get("name") == name]
+    if len(found) != 1 or len(found[0]) != 1:
+        raise ValueError(f"the optimizer needs the reference's single-tensor {name!r} group")
+    return found[0][0]
+
+
+def group_params(optimizer, ordered=False):
+    """{name: parameter} of an optimizer with the reference's six single-tensor groups (NAMES) and no other; ValueError
+    otherwise.  ordered: also in NAMES' order, as a state_dict numbers the groups by position."""
+    got = [g.get("name") for g in optimizer.param_groups]
+    if (got != list(NAMES)) if ordered else (len(got) != len(NAMES) or set(got) != set(NAMES)):
+        raise ValueError(f"the optimizer must have the reference's six single-tensor groups {NAMES}"
+                         f"{' in this order' if ordered else ''}, got {got}")
+    return {k: group_param(optimizer, k) for k in NAMES}
+
+
+def moments(optimizer, p):
+    """(exp_avg, exp_avg_sq) of parameter p, or None before its first step."""
+    st = optimizer.state.get(p)
+    return (st["exp_avg"], st["exp_avg_sq"]) if st is not None and "exp_avg" in st else None
+
+
+def swap_rows(optimizer, new):
+    """Put new rows into the optimizer as the reference's densification does (_prune_optimizer,
+    cat_tensors_to_optimizer, scene/gaussian_model.py:789-881).  new: {group name: (data, (exp_avg, exp_avg_sq) or None)}.
+    Each group gets a NEW nn.Parameter over data; the old parameter's state entry moves to it with the moments replaced
+    when given and every other key ("step") untouched.  -> {group name: new Parameter}."""
+    groups = {g.get("name"): g for g in optimizer.param_groups}
+    out = {}
+    for name, (data, m) in new.items():
+        p = out[name] = nn.Parameter(data)
+        st = optimizer.state.pop(groups[name]["params"][0], None)
+        if st is not None:
+            if m is not None:
+                st["exp_avg"], st["exp_avg_sq"] = m
+            optimizer.state[p] = st
+        groups[name]["params"][0] = p
+    return out
 
 
 class FusedAdam(torch.optim.Optimizer):

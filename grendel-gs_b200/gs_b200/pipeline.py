@@ -19,6 +19,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from .optim import GROUPS
 from .division import (DivisionStrategy, StrategyHistory, finish_strategy, heuristics_update_enabled,  # noqa: F401
                        start_strategy, start_strategy_whole_views)
 
@@ -85,27 +86,27 @@ class GaussianParams(nn.Module):
 
     @classmethod
     def from_raw(cls, raw, device):
-        """The six raw parameters as they are stored (a PLY shard or a checkpoint, model_io): raw = {group name (Trainer.
-        GROUP_OF): tensor}, taken bit for bit, with no activation inverted.  max_sh_degree comes from _features_rest's
+        """The six raw parameters as they are stored (a PLY shard or a checkpoint, model_io): raw = {group name
+        (optim.GROUPS): tensor}, taken bit for bit, with no activation inverted.  max_sh_degree comes from _features_rest's
         (P, (D+1)^2 - 1, 3); active_sh_degree starts at it."""
-        if set(raw) != set(Trainer.GROUP_OF):
-            raise ValueError(f"raw parameters need the groups {sorted(Trainer.GROUP_OF)}, got {sorted(raw)}")
+        if set(raw) != set(GROUPS):
+            raise ValueError(f"raw parameters need the groups {sorted(GROUPS)}, got {sorted(raw)}")
         P = int(raw["xyz"].shape[0])
         for name, tail in cls.RAW_SHAPES.items():
             if tuple(raw[name].shape) != (P,) + tail:
                 raise ValueError(f"raw parameter {name} must be {(P,) + tail}, got {tuple(raw[name].shape)}")
-        Km1 = raw["f_rest"].shape[1] if raw["f_rest"].dim() == 3 else -1
-        if raw["f_rest"].dim() != 3 or tuple(raw["f_rest"].shape) != (P, Km1, 3) or Km1 + 1 not in (1, 4, 9, 16):
-            raise ValueError(f"raw parameter f_rest must be (P, (D+1)^2 - 1, 3) for D = 0..3, got "
-                             f"{tuple(raw['f_rest'].shape)}")
+        rest = tuple(raw["f_rest"].shape)
+        if len(rest) != 3 or rest[0] != P or rest[2] != 3:
+            raise ValueError(f"raw parameter f_rest must be (P, (D+1)^2 - 1, 3) for D = 0..3, got {rest}")
+        max_sh_degree = ops.stored_sh_degree(rest[1] + 1, f"raw parameter f_rest {rest}")
         self = cls.__new__(cls)
         nn.Module.__init__(self)
-        for name, attr in Trainer.GROUP_OF.items():
+        for name, attr in GROUPS.items():
             t = raw[name].detach().to(device=device, dtype=torch.float32)
             if not t.is_contiguous() or t.storage_offset() != 0:   # the kernels need 16-byte aligned, dense rows
                 t = t.clone(memory_format=torch.contiguous_format)
             setattr(self, attr, nn.Parameter(t))
-        self.max_sh_degree = int(round((Km1 + 1) ** 0.5)) - 1
+        self.max_sh_degree = max_sh_degree
         self.active_sh_degree = self.max_sh_degree
         return self
 
@@ -130,7 +131,7 @@ class GaussianParams(nn.Module):
         return torch.cat((self._features_dc, self._features_rest), dim=1)
 
     def raw_parameters(self):
-        return [self._xyz, self._features_dc, self._features_rest, self._scaling, self._rotation, self._opacity]
+        return [getattr(self, attr) for attr in ops.RAW_ORDER]
 
 
 def train_step_single(params, dcam, gt_u8_dev, lambda_dssim=0.2, collector=None, compute_locally=None):
@@ -221,7 +222,7 @@ class Trainer:
         all-gathered on the device and the batch's camera table is gathered there from a resident (N, 40) table, so the
         host never learns the other ranks' views.  The division reads no render times: none are gathered or fed back.
         model: instead of an activated scene (scene=None), this rank's six raw parameters as stored -- {group name
-        (GROUP_OF): tensor}, a shard of a PLY or checkpoint from model_io -- taken bit for bit (GaussianParams.from_raw);
+        (optim.GROUPS): tensor}, a shard of a PLY or checkpoint from model_io -- taken bit for bit (GaussianParams.from_raw);
         max_sh_degree then comes from their shape and the argument is not read.  shard=(lo, hi, n_total) gives the whole
         model's size; without it n_total is this rank's count at world size 1, and their sum over the ranks (one small
         all-reduce) otherwise."""
@@ -1022,18 +1023,17 @@ class Trainer:
         from . import densify
         densify.add_densification_stats(xyz_gradient_accum, denom, max_radii2D, self.means2D.grad, self._radii_local)
 
-    GROUP_OF = {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity",
-                "scaling": "_scaling", "rotation": "_rotation"}
+    GROUP_OF = GROUPS
 
     def optimizer_groups(self, lrs=None):
         """The reference's six single-tensor groups over this trainer's parameters (scene/gaussian_model.py:257-292)."""
         lrs = lrs or {"xyz": 0.00016, "f_dc": 0.0025, "f_rest": 0.0025 / 20, "opacity": 0.05, "scaling": 0.005,
                       "rotation": 0.001}            # arguments/__init__.py:110-119
-        return [{"params": [getattr(self.params, attr)], "lr": lrs[name], "name": name} for name, attr in self.GROUP_OF.items()]
+        return [{"params": [getattr(self.params, attr)], "lr": lrs[name], "name": name} for name, attr in GROUPS.items()]
 
     def adopt_parameters(self, new):
         """After densification / redistribution replaced the optimizer's tensors: new = {group name: nn.Parameter}."""
-        for name, attr in self.GROUP_OF.items():
+        for name, attr in GROUPS.items():
             setattr(self.params, attr, new[name])
         self.n_local = int(new["xyz"].shape[0])
 

@@ -13,11 +13,10 @@ Host-side torch ops (densification is host-side by decree, SURVEY.md 2 #7); the 
 import numpy as np
 import torch
 import torch.distributed as dist
-import torch.nn as nn
 
+from .densify import fresh_stats
 from .exchange import all_to_all_single
-
-NAMES = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation")
+from .optim import NAMES, group_params, moments, swap_rows
 
 
 def fused_rows(tensors, order=None):
@@ -51,10 +50,7 @@ def redistribute(optimizer, destination=None, group=None, generator=None):
     (get_destination_1).  -> dict of the six new parameters + "counts" (i2j_send_size, W x W) + the reset per-Gaussian
     statistics of :1300-1318."""
     W, me = dist.get_world_size(group), dist.get_rank(group)
-    groups = {g["name"]: g for g in optimizer.param_groups}
-    if set(groups) != set(NAMES) or any(len(g["params"]) != 1 for g in groups.values()):
-        raise ValueError("the optimizer must have the reference's six single-tensor groups " + str(NAMES))
-    params = {k: groups[k]["params"][0] for k in NAMES}
+    params = group_params(optimizer)
     P = params["xyz"].shape[0]
     dev = params["xyz"].device
     if destination is None:
@@ -69,39 +65,23 @@ def redistribute(optimizer, destination=None, group=None, generator=None):
     i2j = i2j.reshape(W, W).cpu().numpy()
     send_splits, recv_splits = i2j[me].tolist(), i2j[:, me].tolist()
     # fused rows in send order
-    tensors, widths, has_state = [], [], {}
+    state = {k: moments(optimizer, p) for k, p in params.items()}
     with torch.no_grad():
-        for k in NAMES:
-            st = optimizer.state.get(params[k], None)
-            has_state[k] = st is not None and "exp_avg" in st
-            tensors.append(params[k].detach())
-            if has_state[k]:
-                tensors += [st["exp_avg"], st["exp_avg_sq"]]
+        tensors = [t for k in NAMES for t in (params[k].detach(),) + (state[k] or ())]
         order = torch.sort(destination, stable=True).indices
         send, widths = fused_rows(tensors, order)
         n_new = int(sum(recv_splits))
         recv = torch.empty((n_new, send.shape[1]), dtype=send.dtype, device=dev)
         all_to_all_single(recv, send, recv_splits, send_splits, group)
         del send
-        parts = list(torch.split(recv, widths, dim=1))
-    result, q = {}, 0
+        parts = iter(torch.split(recv, widths, dim=1))
+    new = {}
     for k in NAMES:
-        g, old = groups[k], params[k]
-        new = nn.Parameter(parts[q].reshape((n_new,) + tuple(old.shape[1:])).contiguous().requires_grad_(True))
-        q += 1
-        st = optimizer.state.pop(old, None)
-        if st is not None:
-            if has_state[k]:
-                st["exp_avg"] = parts[q].reshape(new.shape).contiguous()
-                st["exp_avg_sq"] = parts[q + 1].reshape(new.shape).contiguous()
-                q += 2
-            optimizer.state[new] = st
-        g["params"][0] = new
-        result[k] = new
-    result["xyz_gradient_accum"] = torch.zeros((n_new, 1), device=dev)
-    result["denom"] = torch.zeros((n_new, 1), device=dev)
-    result["max_radii2D"] = torch.zeros((n_new,), device=dev)
-    result["sum_visible_count_in_one_batch"] = torch.zeros((n_new,), device=dev)
+        shape = (n_new,) + tuple(params[k].shape[1:])
+        take = lambda: next(parts).reshape(shape).contiguous()   # the next tensor's columns of the received rows
+        new[k] = (take(), None if state[k] is None else (take(), take()))
+    result = swap_rows(optimizer, new)
+    result.update(fresh_stats(n_new, dev))
     result["send_to_gpui_cnt"] = torch.zeros((n_new, W), dtype=torch.int32, device=dev)
     result["counts"] = i2j.tolist()
     return result

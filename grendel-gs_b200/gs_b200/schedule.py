@@ -177,8 +177,8 @@ class Schedule:
                 g["lr"], g["eps"], g["betas"] = float(h["lr"]), float(h["eps"]), tuple(float(b) for b in h["betas"])
             self.optimizer = FusedAdam(groups, lr=0.0, eps=1e-15, grad_scale=grad_scale)
             trainer.params.active_sh_degree = 0
-            self.stats = {"max_radii2D": torch.zeros((P,), device=dev), "xyz_gradient_accum": torch.zeros((P, 1), device=dev),
-                          "denom": torch.zeros((P, 1), device=dev)}
+            fresh = densify.fresh_stats(P, dev)
+            self.stats = {k: fresh[k] for k in model_io.STAT_NAMES}
         else:
             self.optimizer = model_io.load_fused_adam(trainer, checkpoint, grad_scale=grad_scale)
             trainer.params.active_sh_degree = int(checkpoint.active_sh_degree)
