@@ -18,7 +18,7 @@ from types import SimpleNamespace
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import gt_scatter, ops
 from .optim import GROUPS
 from .division import (DivisionStrategy, StrategyHistory, finish_strategy, heuristics_update_enabled,  # noqa: F401
                        start_strategy, start_strategy_whole_views)
@@ -393,24 +393,6 @@ class Trainer:
                              f"camera i where the rank holds it, None elsewhere)")
         self.local_bsz = ks[0]
 
-    # -- ground truth strips (load_camera_from_cpu_to_all_gpu, loss_distribution.py:2395-2533) ------------
-    def _strip_h2d(self, host, y0, y1, cache_key=None):
-        """Rows [y0, y1) of a (3,H,W) uint8 host image -> a (3, rows, W) device strip: the rows of one channel are
-        contiguous in the image, so the strip is three asynchronous copies straight out of a pinned image -- no staging
-        copy, and nothing to re-pin when the load balancer moves the strip boundaries (a pinned staging strip per division
-        cost several ms of cudaHostAlloc every time the strips of a 4K view moved).  A pageable image with a cache_key
-        goes through a pinned copy of the strip kept in the strip cache; without one, the three copies stage through
-        pageable memory."""
-        if not host.is_pinned() and cache_key is not None:
-            key = (cache_key, y0, y1, False)
-            if key not in self._strip_cache:
-                self._strip_cache[key] = host[:, y0:y1, :].contiguous().pin_memory()
-            return self._strip_cache[key].to(self.device, non_blocking=True)
-        d = torch.empty((3, y1 - y0, self.W), dtype=torch.uint8, device=self.device)
-        for c in range(3):
-            d[c].copy_(host[c, y0:y1, :], non_blocking=True)
-        return d
-
     def _mark(self, name):
         """GS_B200_TRACE=1: synchronise and accumulate wall-clock per phase (diagnostics only)."""
         if not self._trace_on:
@@ -531,10 +513,10 @@ class Trainer:
 
     def _eval_args(self, name, views, cams, gts, bsz):
         """The refusals of evaluate / image_metrics, from the arguments alone, before any collective or launch.
-        -> (device cameras, their images, views, bsz, held_out)."""
+        -> (device cameras, their images, views, bsz).  The Trainer's own images are its resident ones, or with
+        distributed_dataset_storage rank 0's host images, scattered."""
         from .exchange import MAX_CAMERAS
-        held_out = cams is not None or gts is not None
-        if held_out:
+        if cams is not None or gts is not None:
             if cams is None or gts is None:
                 raise ValueError(f"{name}: pass cams and gts together (a held-out set), or neither (the Trainer's own)")
             if len(gts) != len(cams):
@@ -556,14 +538,14 @@ class Trainer:
             if (not self.distributed_dataset_storage or self.rank == 0) and any(g is None for g in gts):
                 raise ValueError(f"{name}: a ground-truth image is None (only ranks other than 0 of a "
                                  "distributed_dataset_storage Trainer may leave them out)")
-            host = list(gts)
+            gts = list(gts)
         else:
             if self.gts_dev is None and not self.distributed_dataset_storage:
                 raise ValueError(f"{name}: this Trainer holds no images of its cameras; pass a held-out set")
             if self.local_sampling:
                 raise ValueError(f"{name}: a local-sampling Trainer holds only its own rank's images, so it cannot score "
                                  "its camera set; pass a held-out set (cams=..., gts=...) on every rank")
-            dcams, host = self.dcams, self.gts_host
+            dcams, gts = self.dcams, self.gts_host if self.distributed_dataset_storage else self.gts_dev
         N = len(dcams)
         views = tuple(range(N)) if views is None else tuple(operator.index(v) for v in views)
         if not views:
@@ -577,7 +559,7 @@ class Trainer:
         bsz = operator.index(bsz)
         if not 1 <= bsz <= cap:
             raise ValueError(f"{name}: bsz must be in 1..{cap} at world size {self.world}, got {bsz}")
-        return dcams, host, views, bsz, held_out
+        return dcams, gts, views, bsz
 
     @contextlib.contextmanager
     def _eval_state(self):
@@ -592,77 +574,59 @@ class Trainer:
         finally:
             self._trace_on, ops.STEP_STREAM = saved
 
-    def _eval_batches(self, dcams, host, views, bsz, held_out):
+    def _eval_batches(self, dcams, gts, views, bsz):
         """The batches of an evaluation, bsz views each: a fresh strip division of the listed views (one history per
-        call), each local strip's ground truth, and the forward.  Yields (strategies, rows, gts, gt_row0, fw) per batch:
-        rows[k] the local pixel rows of view k ((0, 0): none); gts[k] a device image holding rows [gt_row0[k], ...) of its
-        ground truth -- a resident image in place, or a strip -- or None; fw the _forward namespace."""
+        call), each local strip's ground truth, and the forward.  Yields (strategies, rows, pairs, fw) per batch: rows[k]
+        the local pixel rows of view k ((0, 0): none); pairs[k] its ground truth as gt_scatter.local_gt gives it, None or
+        (tensor, row0); fw the _forward namespace."""
         p, H = self.params, self.H
         history = StrategyHistory(sorted({dcams[v].uid for v in views}), self.tile_y, self.world)
         for b0 in range(0, len(views), bsz):
             bviews = views[b0:b0 + bsz]
             bcams = [dcams[v] for v in bviews]
-            strategies, tasks = start_strategy([c.uid for c in bcams], history, self.world, self.rank)
+            strategies = start_strategy([c.uid for c in bcams], history, self.world, self.rank)[0]
             settings = [c.settings(p.active_sh_degree) for c in bcams]
-            # each local strip's ground truth and its first row: resident images in place, host images by strip rows
-            gts, gt_row0, rows = [], [], []
-            if self.distributed_dataset_storage:
-                from . import gt_scatter
-                strips, _ = gt_scatter.scatter_gt_strips([host[v] for v in bviews] if self.rank == 0 else self.W, tasks,
-                                                         H, self.device, self.rank, self.world, self.group)
-            for k, st in enumerate(strategies):
-                r = st.local_pixel_rows(H)
-                if r is None:
-                    gts.append(None); gt_row0.append(0); rows.append((0, 0))
-                    continue
-                rows.append(r)
-                if self.distributed_dataset_storage:
-                    gts.append(strips[k]); gt_row0.append(r[0])
-                elif not held_out:
-                    gts.append(self.gts_dev[bviews[k]]); gt_row0.append(0)
-                elif host[bviews[k]].is_cuda:
-                    gts.append(host[bviews[k]]); gt_row0.append(0)
-                else:
-                    gts.append(self._strip_h2d(host[bviews[k]], r[0], r[1])); gt_row0.append(r[0])
+            pairs = gt_scatter.local_gt(gts, bviews, strategies, H, self.W, self.device, self.rank, self.world,
+                                        self.group, scatter=self.distributed_dataset_storage)[0]
+            rows = [st.local_pixel_rows(H) or (0, 0) for st in strategies]
             fw = self._forward(settings[0], strategies, {}, lambda: ops.pack_cameras(settings), (0, len(bcams)),
                                training=False)
-            yield strategies, rows, gts, gt_row0, fw
+            yield strategies, rows, pairs, fw
 
-    def _sum_slots_over_ranks(self, slots):
+    def _per_view(self, slots, finalize):
+        """The slots of every batch summed over the ranks in ONE all-reduce and finalized batch by batch on the device.
+        -> ((n, 2) per-view values, their means over the views as floats: the call's one host read)."""
+        sizes = [s.shape[0] for s in slots]
+        slots = torch.cat(slots) if len(slots) > 1 else slots[0]
         if self.world > 1:   # every tile row is non-zero on one rank only: the sum is exact in any order
             import torch.distributed as dist
             dist.all_reduce(slots, op=dist.ReduceOp.SUM, group=self.group)
-        return slots
-
-    def _evaluate(self, dcams, host, views, bsz, held_out):
-        batches, slots = [], []
-        for strategies, rows, gts, gt_row0, fw in self._eval_batches(dcams, host, views, bsz, held_out):
-            slots.append(ops.eval_sums_batched(fw.images, gts, rows, gt_row0))
-            batches.append(len(strategies))
-        slots = self._sum_slots_over_ranks(torch.cat(slots) if len(slots) > 1 else slots[0])
-        per_view, b0 = [], 0
-        for b in batches:
-            per_view.append(ops.eval_finalize(slots[b0:b0 + b], self.H, self.W))
-            b0 += b
+        per_view = [finalize(s, self.H, self.W) for s in slots.split(sizes)]
         per_view = torch.cat(per_view) if len(per_view) > 1 else per_view[0]
-        means = (per_view.sum(0) / len(views)).tolist()   # the call's one host read
+        return per_view, (per_view.sum(0) / per_view.shape[0]).tolist()
+
+    def _evaluate(self, dcams, gts, views, bsz):
+        slots = [ops.eval_sums_batched(fw.images, [None if g is None else g[0] for g in pairs], rows,
+                                       [0 if g is None else g[1] for g in pairs])
+                 for _, rows, pairs, fw in self._eval_batches(dcams, gts, views, bsz)]
+        per_view, means = self._per_view(slots, ops.eval_finalize)
         return {"l1": means[0], "psnr": means[1], "l1_per_view": per_view[:, 0], "psnr_per_view": per_view[:, 1]}
 
-    def _image_metrics(self, dcams, host, views, bsz, held_out, images):
+    def _image_metrics(self, dcams, gts, views, bsz, images):
         from . import image_halo
         H, W = self.H, self.W
-        batches, slots, pictures = [], [], []
-        for strategies, rows, gts, gt_row0, fw in self._eval_batches(dcams, host, views, bsz, held_out):
+        slots, pictures = [], []
+        for strategies, rows, pairs, fw in self._eval_batches(dcams, gts, views, bsz):
             # per local strip a (6, rows, W) window of the strip and its halo: 8-bit render in channels 0-2, ground truth
             # in 3-5; the strip's own rows filled here, the halo rows by the neighbours' owners
             wins, win_row0 = [], []
-            for k, (y0, y1) in enumerate(rows):
-                if y1 == y0:
+            for (y0, y1), g in zip(rows, pairs):
+                if g is None:
                     wins.append(None); win_row0.append(0)
                     continue
-                a, b = image_halo.window_rows((y0, y1), H)
+                (gt, row0), (a, b) = g, image_halo.window_rows((y0, y1), H)
                 win = torch.empty((6, b - a, W), dtype=torch.uint8, device=self.device)
-                win[3:, y0 - a:y1 - a].copy_(gts[k][:, y0 - gt_row0[k]:y1 - gt_row0[k]])
+                win[3:, y0 - a:y1 - a].copy_(gt[:, y0 - row0:y1 - row0])
                 wins.append(win); win_row0.append(a)
             ops.quantize_u8_batched(fw.images, rows, [None if w is None else w[:3] for w in wins], win_row0)
             if self.world > 1:
@@ -671,20 +635,13 @@ class Trainer:
                 slots.append(ops.image_metric_sums_batched(wins, win_row0, rows, H))
             else:   # no strip of this batch here: every slot is +0.0
                 slots.append(torch.zeros((len(rows), self.tile_y, 2), dtype=torch.float64, device=self.device))
-            batches.append(len(strategies))
             if images:
                 strips = [None if w is None else w[:3, y0 - a:y1 - a]
                           for w, a, (y0, y1) in zip(wins, win_row0, rows)]
                 got = image_halo.gather_images(strips, strategies, H, W, self.rank, self.world, self.group, self.device)
                 if got is not None:
                     pictures.extend(got)
-        slots = self._sum_slots_over_ranks(torch.cat(slots) if len(slots) > 1 else slots[0])
-        per_view, b0 = [], 0
-        for b in batches:
-            per_view.append(ops.image_metric_finalize(slots[b0:b0 + b], H, W))
-            b0 += b
-        per_view = torch.cat(per_view) if len(per_view) > 1 else per_view[0]
-        means = (per_view.sum(0) / len(views)).tolist()   # the call's one host read; the image copies are complete too
+        per_view, means = self._per_view(slots, ops.image_metric_finalize)   # the image copies are complete too
         return {"ssim": means[0], "psnr": means[1], "ssim_per_view": per_view[:, 0], "psnr_per_view": per_view[:, 1],
                 "images": pictures if images and (self.rank == 0 or self.world == 1) else None}
 
@@ -795,32 +752,25 @@ class Trainer:
         p = self.params
         for t in p.raw_parameters():
             t.grad = None
-        self._h2d = 0
         strategies, cam_table, (lo, hi), feedback = self._step_plan(views)
         rs = self.dcams[views[0]].settings(p.active_sh_degree)   # image size and background, shared by every view
-        # "Asynchronously load ground-truth image to GPU" (loss_distribution.py:2399): the strips this rank needs are
-        # copied from pinned host memory on a side stream while preprocess / binning / blend run, and the loss waits
-        # on the copy's event.
-        gt_ready = {}
-        if not resident and self.distributed_dataset_storage:
-            from . import gt_scatter
-            tasks = [[(k, st.division_pos[st.gpu_ids.index(g)], st.division_pos[st.gpu_ids.index(g) + 1])
-                      for k, st in enumerate(strategies) if g in st.gpu_ids] for g in range(self.world)]
-            batch_host = [self.gts_host[i] for i in views] if self.rank == 0 else self.W
-            strips, h2d = gt_scatter.scatter_gt_strips(batch_host, tasks, self.H, self.device, self.rank, self.world,
-                                                       self.group)
-            self._h2d += h2d
-            ev = torch.cuda.Event()
-            ev.record(torch.cuda.current_stream())
-            gt_ready = {k: (t, ev) for k, t in strips.items()}
-        elif not resident:
-            for k, st in enumerate(strategies[lo:hi]):
-                rows = st.local_pixel_rows(self.H)
-                if rows is not None:
-                    gt_ready[k] = self._copy_gt(views[k], rows[0], rows[1])
+        # "Asynchronously load ground-truth image to GPU" (loss_distribution.py:2399): host strips are copied on a side
+        # stream while preprocess / binning / blend run, and the loss waits for them
+        if not resident and self._copy_stream is None:
+            self._copy_stream = torch.cuda.Stream(device=self.device)
+        gt, self._h2d, ready = gt_scatter.local_gt(
+            self.gts_dev if resident else self.gts_host, views, strategies[lo:hi], self.H, self.W, self.device,
+            self.rank, self.world, self.group, scatter=self.distributed_dataset_storage and not resident,
+            cache=self._strip_cache, stream=None if resident else self._copy_stream)
         collectors = [{} for _ in range(hi - lo)]
         fw = self._forward(rs, strategies, collectors[0], cam_table, (lo, hi), training=True, feedback=feedback)
         self.means2D, self._radii_local = fw.means2D, fw.radii
+        if ready is not None:
+            cur = torch.cuda.current_stream()
+            cur.wait_event(ready)
+            for g in gt:
+                if g is not None:
+                    g[0].record_stream(cur)
         if self.border_exchange:
             # the legacy row L1: one loss per local strip, summed in view order; a strip of a view split over several
             # ranks is widened by the 5 halo rows its neighbours render, so the strip losses sum to the full-image loss.
@@ -828,31 +778,27 @@ class Trainer:
             # launch, dot with (1 - lambda, -lambda), + lambda), so the loss and gradients keep their bits.
             loss_sum, pairs = None, []
             for k, st in enumerate(strategies):
-                rows = st.local_pixel_rows(self.H)
-                if rows is None:
+                if gt[k] is None:
                     continue
+                rows = st.local_pixel_rows(self.H)
                 if len(st.gpu_ids) > 1:
                     from . import border
                     image, (r0, r1), _ = border.add_remote_border_rows(fw.images[k], st, self.H, self.group)
-                    gt, rows4, gt_full = self.gts_dev[views[k]], (r0, r1, *rows), True
-                else:
-                    image, rows4 = fw.images[k], (*rows, *rows)
-                    gt = self.gts_dev[views[k]] if resident else self._wait_gt(gt_ready[k])
-                    gt_full = resident and rows != (0, self.H)
-                pair = ops.fused_l1_ssim_batched(image[None], [gt], [rows4], deterministic=self.deterministic,
+                    g, rows4, gt_full = self.gts_dev[views[k]], (r0, r1, *rows), True
+                else:   # the view is this rank's alone, so its strip is every row: the strip form
+                    image, rows4, g, gt_full = fw.images[k], (*rows, *rows), gt[k][0], False
+                pair = ops.fused_l1_ssim_batched(image[None], [g], [rows4], deterministic=self.deterministic,
                                                  gt_full=gt_full)
                 pairs.append((k, pair))
                 loss = torch.dot(pair.reshape(-1), self._loss_w) + float(self.lambda_dssim)
                 loss_sum = loss if loss_sum is None else loss_sum + loss
             self._record_losses(views, len(strategies), strips=pairs)
         else:
-            gts = [None if y1 == y0 else self.gts_dev[views[k]] if resident else self._wait_gt(gt_ready[k])
-                   for k, (y0, y1, _c0, _c1) in enumerate(fw.rows4)]
             # the resident image of a one-view batch that is local whole is read as a strip of every row (no host-side
             # row tables); every other resident image is read in place at its strip rows
             gt_full = resident and not (len(views) == 1 and fw.rows4[0] == (0, self.H, 0, self.H))
-            l1_ssim = ops.fused_l1_ssim_batched(fw.images, gts, fw.rows4, deterministic=self.deterministic,
-                                                gt_full=gt_full)
+            l1_ssim = ops.fused_l1_ssim_batched(fw.images, [None if g is None else g[0] for g in gt], fw.rows4,
+                                                deterministic=self.deterministic, gt_full=gt_full)
             # sum over the local strips of (1 - lambda) Ll1 + lambda (1 - ssim)
             loss_sum = torch.dot(l1_ssim.reshape(-1), fw.coef) + fw.const
             self._record_losses(views, len(strategies), span=(lo, hi), l1_ssim=l1_ssim)
@@ -873,26 +819,6 @@ class Trainer:
         self.iteration += 1
         if feedback:
             self._feed_back_times(strategies, collectors)
-
-    def _copy_gt(self, view, y0, y1):
-        """Rows [y0, y1) of a view's host image, copied on the side stream while preprocess / binning / blend run.
-        -> (device strip, the copy's event) for _wait_gt."""
-        if self._copy_stream is None:
-            self._copy_stream = torch.cuda.Stream(device=self.device)
-        with torch.cuda.stream(self._copy_stream):
-            d = self._strip_h2d(self.gts_host[view], y0, y1, cache_key=view)
-            self._h2d += d.numel()
-            ev = torch.cuda.Event()
-            ev.record(self._copy_stream)
-        return d, ev
-
-    @staticmethod
-    def _wait_gt(ready):
-        """The device strip of a (strip, event) pair, once the current stream has waited for its copy."""
-        gt, ev = ready
-        torch.cuda.current_stream().wait_event(ev)
-        gt.record_stream(torch.cuda.current_stream())
-        return gt
 
     def _preprocess(self, rs, cam_table, B, training):
         """This rank's Gaussians projected into the B views of a batch -> (means2D (B,P,2), rgb, conic_opacity, radii,

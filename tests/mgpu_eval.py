@@ -4,7 +4,8 @@
         tests/mgpu_eval.py
 
 W ranks, each holding its shard of the scene, evaluate the camera set and a held-out set with pipeline.Trainer.evaluate at
-several batch sizes, over the peer-memory exchange and over all_to_all_single (peer_exchange=False).  A one-rank Trainer
+several batch sizes, over the peer-memory exchange and over all_to_all_single (peer_exchange=False), and with
+distributed_dataset_storage=True, where only rank 0 holds the images and scatters each rank's strips.  A one-rank Trainer
 over the whole scene on rank 0 is the reference: every view's L1 and PSNR must be the same bits.  The slots of a view are
 non-zero on the one rank that owns each tile row, so their all-reduce is exact; the renders of the strips are those of
 the whole view, so the sums are too."""
@@ -24,14 +25,17 @@ from gs_b200 import pipeline, synthetic as syn  # noqa: E402
 W_IMG, H_IMG, N_CAMS, N_GAUSS = 320, 264, 12, 30000
 
 
-def check(dev, rank, world, peer, log=print):
+def check(dev, rank, world, peer, dds=False, log=print):
     n = N_GAUSS - N_GAUSS % world
     scene = syn.make_scene(n, W_IMG, H_IMG, seed=21, radius_px=8.0)
     cams = [syn.make_camera(W_IMG, H_IMG, yaw_deg=3.0 * q - 15.0, uid=q) for q in range(N_CAMS)]
     gts = [torch.from_numpy(syn.make_gt_image(W_IMG, H_IMG, seed=50 + q)).pin_memory() for q in range(N_CAMS)]
     held_cams = [syn.make_camera(W_IMG, H_IMG, yaw_deg=2.0 * q - 9.0, uid=100 + q) for q in range(5)]
     held_gts = [torch.from_numpy(syn.make_gt_image(W_IMG, H_IMG, seed=80 + q)) for q in range(5)]
-    tr = pipeline.Trainer(scene, cams, gts, dev, rank, world, load_balance=False, peer_exchange=peer)
+    if dds:   # only rank 0 holds the images, its own and the held-out ones
+        gts, held_gts = [g if rank == 0 else None for g in gts], [g if rank == 0 else None for g in held_gts]
+    tr = pipeline.Trainer(scene, cams, None if dds and rank != 0 else gts, dev, rank, world, load_balance=False,
+                          peer_exchange=peer, distributed_dataset_storage=dds)
     one = pipeline.Trainer(scene, cams, gts, dev) if rank == 0 else None
     ok = True
     for what, kw, views in (("own", {}, [4, 0, 11, 7, 7, 2, 9]), ("held-out", dict(cams=held_cams, gts=held_gts),
@@ -42,7 +46,8 @@ def check(dev, rank, world, peer, log=print):
                 want = one.evaluate(views, **kw)
                 same = (torch.equal(got["l1_per_view"], want["l1_per_view"]) and
                         torch.equal(got["psnr_per_view"], want["psnr_per_view"]))
-                log(f"[mgpu-eval] world {world} {'peer' if peer else 'nccl'} {what} bsz {bsz}: L1 {got['l1']:.9f} "
+                log(f"[mgpu-eval] world {world} {'peer' if peer else 'nccl'}{' dataset on rank 0' if dds else ''} {what} "
+                    f"bsz {bsz}: L1 {got['l1']:.9f} "
                     f"PSNR {got['psnr']:.6f} vs one rank {want['l1']:.9f} / {want['psnr']:.6f}: "
                     f"{'bit-exact' if same else 'DIFFERENT'}")
                 ok = ok and same
@@ -60,7 +65,7 @@ def main():
     dev = torch.device("cuda", local)
     dist.init_process_group("nccl", device_id=dev)
     log = (lambda m: print(m, flush=True)) if rank == 0 else (lambda m: None)
-    ok = all([check(dev, rank, world, peer, log=log) for peer in (True, False)])
+    ok = all([check(dev, rank, world, peer, dds, log=log) for peer, dds in ((True, False), (False, False), (True, True))])
     log(f"[mgpu-eval] {'PASS' if ok else 'FAIL'} world_size {world}")
     dist.barrier()
     dist.destroy_process_group()

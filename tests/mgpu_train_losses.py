@@ -11,7 +11,10 @@ loss] with a one-rank Trainer over the whole scene stepping the same views:
   * the strip division without it: Ll1 within the same bound; the SSIM of a split view sees the strip edges, as the
     reference's strip loss does, so its difference is only reported;
   * local sampling (each rank draws local_bsz views of the images it holds; the batch is the ranks' views in rank order):
-    every view is rendered whole by one rank, within the same bound (whether it is bit for bit is reported).
+    every view is rendered whole by one rank, within the same bound (whether it is bit for bit is reported);
+  * distributed_dataset_storage=True (only rank 0 holds the images and scatters each rank's strips), with and without
+    border_exchange: every resident=False step's loss and gradients, and the drained entries, are the bits of the default
+    Trainer at the same world size.
 Every rank's drained entries must be the same (the records are summed over the ranks)."""
 import os
 import sys
@@ -87,6 +90,30 @@ def check_division(dev, rank, world, border, steps=4, log=print):
     return bool(flag.item() > 0)
 
 
+def check_dataset_storage(dev, rank, world, border, steps=4, log=print):
+    scene, cams, gts = scene_of(world)
+    kw = dict(lambda_dssim=LAM, deterministic=True, load_balance=False, border_exchange=border)
+    # border_exchange reads the strips of views split over several ranks from every rank's resident images
+    tr = pipeline.Trainer(scene, cams, gts if rank == 0 or border else None, dev, rank, world,
+                          distributed_dataset_storage=True, **kw)
+    ref = pipeline.Trainer(scene, cams, gts, dev, rank, world, **kw)
+    rng = np.random.default_rng(9)
+    same = True
+    for _ in range(steps):
+        views = [int(v) for v in rng.choice(N_CAMS, size=int(rng.integers(1, 9)))]
+        a, b = tr.step(views=views, resident=False), ref.step(views=views, resident=False)
+        same = same and np.float32(a).view(np.int32) == np.float32(b).view(np.int32)
+        same = same and all(torch.equal(x.grad.view(torch.int32), y.grad.view(torch.int32))
+                            for x, y in zip(tr.params.raw_parameters(), ref.params.raw_parameters()))
+    same = same and tr.train_losses() == ref.train_losses()
+    flag = torch.tensor([1.0 if same else 0.0], device=dev)
+    dist.all_reduce(flag, op=dist.ReduceOp.MIN)
+    ok = bool(flag.item() > 0)
+    log(f"[mgpu-tl] world {world} distributed_dataset_storage, border_exchange={border}: "
+        f"{'bit-exact' if ok else 'DIFFERENT'} against the default Trainer")
+    return ok
+
+
 def check_local_sampling(dev, rank, world, local_bsz, steps=3, log=print):
     scene, cams, gts = scene_of(world)
     held = [g if q % world == rank else None for q, g in enumerate(gts)]
@@ -121,6 +148,7 @@ def main():
     log = (lambda m: print(m, flush=True)) if rank == 0 else (lambda m: None)
     results = [check_division(dev, rank, world, border, log=log) for border in (True, False)]
     results += [check_local_sampling(dev, rank, world, k, log=log) for k in (1, 2)]
+    results += [check_dataset_storage(dev, rank, world, border, log=log) for border in (True, False)]
     ok = all(results)
     log(f"[mgpu-tl] {'PASS' if ok else 'FAIL'} world_size {world}")
     dist.barrier()

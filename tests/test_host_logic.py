@@ -254,6 +254,23 @@ def test_layout_is_consistent_without_a_group():
         assert pos == lays[a].total_send
 
 
+class _Pinned(torch.Tensor):
+    """A pinned host image, without a driver to pin it."""
+    def is_pinned(self, *args, **kwargs):
+        return True
+
+
+class _Pageable(torch.Tensor):
+    """A pageable host image; pin_memory() needs a driver, so the strip cache's pinned copy is a plain copy here."""
+    def pin_memory(self, *args, **kwargs):
+        return self.clone()
+
+
+class _OnDevice(torch.Tensor):
+    """An image already on the step's device."""
+    is_cuda = property(lambda self: True)
+
+
 def _gt_scatter_worker(rank, world, port, q):
     import torch.distributed as dist
     from gs_b200 import gt_scatter
@@ -261,12 +278,44 @@ def _gt_scatter_worker(rank, world, port, q):
     H, W, B, tile_y = 100, 40, 3, 7
     gts = [torch.from_numpy(np.random.default_rng(k).integers(0, 256, (3, H, W), dtype=np.uint8)) for k in range(B)]
     hist = division.StrategyHistory(list(range(B)), tile_y, world)
-    _, tasks = division.start_strategy(list(range(B)), hist, world, rank)
+    strategies, tasks = division.start_strategy(list(range(B)), hist, world, rank)
     got, h2d = gt_scatter.scatter_gt_strips(gts if rank == 0 else W, tasks, H, "cpu", rank, world)
-    ok = set(got) == {t[0] for t in tasks[rank]}
+    ok = set(got) == {t[0] for t in tasks[rank]} and gt_scatter.strip_tasks(strategies, world) == tasks
     for cam, l, r in tasks[rank]:
         y0, y1 = l * 16, min(r * 16, H)
         ok = ok and torch.equal(got[cam], gts[cam][:, y0:y1, :])
+
+    # local_gt: batch position k is camera views[k]; every source gives its local rows [y0, y1) at the expected row0
+    views = [2, 0, 1]
+    local = {k: st.local_pixel_rows(H) for k, st in enumerate(strategies) if st.local_rows() is not None}
+    strip_bytes = sum(3 * (y1 - y0) * W for y0, y1 in local.values())
+
+    def same(pairs, in_place):
+        good = len(pairs) == B and all(pairs[k] is None for k in range(B) if k not in local)
+        for k, (y0, y1) in local.items():
+            t, row0 = pairs[k]
+            want = gts[views[k]][:, y0:y1, :]
+            good = good and row0 == (0 if in_place else y0) and torch.equal(t[:, y0 - row0:y1 - row0, :], want)
+            good = good and (t is images[views[k]] if in_place else tuple(t.shape) == tuple(want.shape))
+        return good
+
+    for source in ("scatter", "pinned", "pageable", "held-out", "in place"):
+        cache = None if source == "held-out" else {}
+        cls = {"pinned": _Pinned, "pageable": _Pageable, "in place": _OnDevice}.get(source)
+        images = [g if cls is None else g.as_subclass(cls) for g in gts]
+        if source == "scatter" and rank != 0:
+            images = None
+        pairs, n, ready = gt_scatter.local_gt(images, views, strategies, H, W, "cpu", rank, world,
+                                              scatter=source == "scatter", cache=cache)
+        ok = ok and ready is None and same(pairs, source == "in place")
+        if source == "scatter":
+            ok = ok and n == (h2d if rank == 0 else 0)
+        else:
+            ok = ok and n == (0 if source == "in place" else strip_bytes)
+        if source == "pageable":   # the own set's pageable strips stay cached, keyed by camera and rows
+            ok = ok and set(cache) == {(views[k], y0, y1) for k, (y0, y1) in local.items()}
+        elif cache is not None:
+            ok = ok and cache == {}
     q.put((rank, bool(ok), h2d))
     dist.barrier()
     dist.destroy_process_group()
@@ -275,7 +324,10 @@ def _gt_scatter_worker(rank, world, port, q):
 @pytest.mark.parametrize("world", [2, 3])
 def test_gt_strips_scattered_from_rank0_match_the_local_slices(world):
     """loss_distribution.py:2395-2533 with --distributed_dataset_storage: only rank 0 holds pixels; every rank ends up
-    with exactly the uint8 rows of its strips (3 cameras over 2 / 3 ranks: strips that start and end mid-image)."""
+    with exactly the uint8 rows of its strips (3 cameras over 2 / 3 ranks: strips that start and end mid-image).
+    gt_scatter.local_gt, which every training step and evaluation reads its ground truth through, gives each batch
+    position's strip rows from each source -- the scatter, pinned and pageable host images (the latter through the
+    strip cache, held-out ones without it) and images on the device read in place -- with the expected first row."""
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
