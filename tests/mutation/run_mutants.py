@@ -1,8 +1,8 @@
-"""Mutation runner for the projection and blend kernels: which deliberately wrong kernel does the suite let through?
+"""Mutation runner for the kernels of catalogue.py: which deliberately wrong kernel does the suite let through?
 
     python tests/mutation/run_mutants.py --build            # no GPU needed: nvcc cross-compiles
     python tests/mutation/run_mutants.py --run [--jobs N]   # on an H100; writes the kill matrix (JSON)
-    python tests/mutation/run_mutants.py --merge a.json,b.json --out m.json   # combine runs over parts of the selection
+    python tests/mutation/run_mutants.py --merge a.json,b.json --out m.json   # combine runs (and earlier merged matrices)
 
 --build copies csrc/ (with include/) once per mutant of catalogue.py into tests/mutation/build/<id>/ (git-ignored), applies that one
 mutant (its original snippet must occur exactly once), compiles only the mutated .cu with the flags of
@@ -201,26 +201,24 @@ def _summary(cat, rows):
 
 def merge(cat, paths, out_path):
     """One kill matrix from runs over parts of the selection (e.g. --before-only, then --after-only): a mutant's
-    verdicts per file are combined, killed_before comes from the BEFORE files alone."""
-    rows, baselines = {}, []
+    verdicts per file are combined, killed_before comes from the BEFORE files alone.  A path may also be an earlier
+    merged matrix: its runs and rows are carried over as they are."""
+    rows, runs = {}, []
     for p in paths:
         with open(p) as f:
             d = json.load(f)
-        baselines.append(d["baseline"])
+        runs += d["runs"] if "runs" in d else [dict(baseline=d["baseline"], summary=d["summary"])]
         for r in d["mutants"]:
             row = rows.setdefault(r["id"], dict(r, killed_by={}, seconds=0.0))
             row["killed_by"].update(r["killed_by"])
             row["seconds"] = round(row["seconds"] + r["seconds"], 1)
     for row in rows.values():
+        row["equivalent"] = cat.EQUIVALENT.get(row["id"])   # the catalogue's current verdict
         before = set(cat.SELECTION[row["file"]]["BEFORE"])
         row["killed_before"] = any(v for f, v in row["killed_by"].items() if f in before)
         row["killed"] = any(row["killed_by"].values())
     order = {m.id: i for i, m in enumerate(cat.MUTANTS)}
-    result = dict(runs=[dict(baseline=b, summary=None) for b in baselines],
-                  mutants=sorted(rows.values(), key=lambda r: order[r["id"]]))
-    for run, p in zip(result["runs"], paths):
-        with open(p) as f:
-            run["summary"] = json.load(f)["summary"]
+    result = dict(runs=runs, mutants=sorted(rows.values(), key=lambda r: order[r["id"]]))
     result["summary"] = _summary(cat, result["mutants"])
     with open(out_path, "w") as f:
         json.dump(result, f, indent=1)
